@@ -7,7 +7,7 @@ import os
 from ctypes import c_char_p, c_double, c_float, c_int, c_int64, c_void_p
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("B200SEG_LIB") or os.path.join(HERE, "libb200seg.so")      # B200SEG_LIB: the instrumented twin (build.py --profile)
+LIB_PATH = os.path.join(HERE, "libb200seg.so")
 
 F32, F16 = 0, 1
 ALGO_AUTO, ALGO_DIRECT, ALGO_TC = 0, 1, 2

@@ -20,24 +20,17 @@ def _stale():
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
 
-def build(force=False, verbose=False, profile=False):
-    """Compile every .cu into objects (parallel) and link the shared library.  profile=True builds the instrumented
-    twin libb200seg_prof.so (-DB200SEG_TC_PROFILE: per-wait-site cycle counters in the tensor-core kernels, read and reset
-    through b200seg_conv_tc_prof / b200seg_wgrad_tc_prof)."""
-    if profile:
-        return _build(os.path.join(HERE, "libb200seg_prof.so"), os.path.join(HERE, "build_prof"), ["-DB200SEG_TC_PROFILE"], verbose)
+def build(force=False, verbose=False):
+    """Compile every .cu into objects (parallel) and link the shared library."""
     if not force and not _stale():
         return LIB
-    return _build(LIB, os.path.join(HERE, "build"), [], verbose)
-
-
-def _build(LIB, objdir, extra, verbose):
     nvcc = os.environ.get("NVCC", "nvcc")
+    objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
     procs = []
     for src in SOURCES:
         obj = os.path.join(objdir, src.replace(".cu", ".o"))
-        cmd = [nvcc, *NVCC_FLAGS, *extra, "-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [nvcc, *NVCC_FLAGS, "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             print(" ".join(cmd))
         procs.append((src, obj, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
@@ -57,4 +50,4 @@ def _build(LIB, objdir, extra, verbose):
 
 
 if __name__ == "__main__":
-    print(build(force="--force" in sys.argv, verbose=True, profile="--profile" in sys.argv))
+    print(build(force="--force" in sys.argv, verbose=True))

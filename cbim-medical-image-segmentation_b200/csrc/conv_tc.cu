@@ -29,7 +29,6 @@
 #include "tmap.h"
 #include "wgmma.cuh"
 #include <string.h>
-#include <stdlib.h>
 
 namespace {
 
@@ -61,6 +60,17 @@ struct TcParams {
   int use_tma;             // halo tiles are staged by ONE tensor-TMA box per stage (else 16-byte cp.async copies)
   int smem_a_off, smem_b_off, smem_bar_off, smem_norm_off, smem_gnorm_off;
   alignas(64) CUtensorMap tm_x;      // x as {8 ch, w, h, channel plane, b*D + d}
+};
+
+// barrier block layout (uint64 each): a_full[SA] a_empty[SA] b_full[SB] b_empty[SB] a_land[SA].  SA / SB are read from
+// the kernel parameters, not copied: copies would hold registers in every role (measured: more loader spills).
+struct Bars {
+  uint32_t bar0; const TcParams& p;
+  __device__ __forceinline__ uint32_t a_full(int i) const { return bar0 + 8u * (uint32_t)i; }
+  __device__ __forceinline__ uint32_t a_empty(int i) const { return bar0 + 8u * (uint32_t)(p.SA + i); }
+  __device__ __forceinline__ uint32_t b_full(int i) const { return bar0 + 8u * (uint32_t)(2 * p.SA + i); }
+  __device__ __forceinline__ uint32_t b_empty(int i) const { return bar0 + 8u * (uint32_t)(2 * p.SA + p.SB + i); }
+  __device__ __forceinline__ uint32_t a_land(int i) const { return bar0 + 8u * (uint32_t)(2 * p.SA + 2 * p.SB + i); }   // TMA: the stage's box has landed
 };
 
 struct TileCoord { int b, d, h0, w0, ntile; };
@@ -122,28 +132,13 @@ struct StageCursor {
 // later transforms exactly those chunks, so no cross-thread synchronisation is needed between copy and transform.
 // Everything that does not depend on the tile (voxel slot, offset from the tile origin, halo row / column) is computed
 // once per thread; per stage the work is one pointer add per chunk, and the bounds tests vanish for interior tiles.
-constexpr int kMaxChunks = 6;      // ceil(180 halo voxels / (256 threads / (KC/8) planes)) for KC <= 64
-
-// normalise + activate three 8-channel chunks held in registers.  Straight-line on purpose: the three dependency chains
-// interleave (the bounds tests only predicate the shared-memory load and store around this)
-template <bool RELU>
-__device__ __forceinline__ void transform3(uint4 (&raw)[3], const float (&sc)[8], const float (&sf)[8], float slope) {
-#pragma unroll
-  for (int u = 0; u < 3; ++u) {
-    __half2* hv = reinterpret_cast<__half2*>(&raw[u]);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float2 f = __half22float2(hv[j]);
-      f.x = fmaf(f.x, sc[2 * j], sf[2 * j]); f.y = fmaf(f.y, sc[2 * j + 1], sf[2 * j + 1]);
-      if (RELU) { f.x = fmaxf(f.x, 0.f); f.y = fmaxf(f.y, 0.f); }
-      else { f.x = act_apply_s(f.x, slope); f.y = act_apply_s(f.y, slope); }
-      hv[j] = __floats2half2_rn(f.x, f.y);
-    }
-  }
-}
+constexpr int kMaxChunks = 6;
+// the chunk table covers every halo tile: kh, kw <= 3 (conv3d_tc_shape_ok) and KC <= 64 (tc_pick_kc), so at most
+// 18 x 10 halo voxels over at least 256 / 8 threads per plane
+static_assert(kMaxChunks * (kLoadThreads / (64 / 8)) >= (TH + 2) * (TW + 2), "loader chunk table smaller than the largest halo tile");
 
 template <int P, bool TMA>
-__device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, const float2* s_norm, uint32_t bar0) {
+__device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, const float2* s_norm, const Bars& bars) {
   const ConvArgs& a = p.a;
   const int lt = threadIdx.x - kLoadWarp0 * 32;
   const int cpv = p.KC / 8;
@@ -156,9 +151,6 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
   const __half* xbase = reinterpret_cast<const __half*>(a.x);
   const uint32_t smem_a = smem_u32(smem + p.smem_a_off) + (uint32_t)(c8 * p.plane_stride);
   uint8_t* smem_a_gen = smem + p.smem_a_off + c8 * p.plane_stride;
-  auto A_FULL = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-  auto A_EMPTY = [&](int i) { return bar0 + 8u * (uint32_t)(p.SA + i); };
-  auto A_LAND = [&](int i) { return bar0 + 8u * (uint32_t)(2 * p.SA + 2 * p.SB + i); };
   // TMA mode: thread 0 stages the halo tile with ONE tensor-TMA box per stage; every thread then transforms exactly
   // the chunks it would have copied (same table, same code) once the box has landed.  Nobody but thread 0 walks the
   // issue cursor.
@@ -190,14 +182,14 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
   auto issue = [&]() {
     if constexpr (TMA) {
       if (lt == 0) {
-        mbar_wait(A_EMPTY(ri.idx), ri.phase ^ 1, 1);
-        mbar_arrive_expect_tx(A_LAND(ri.idx), stage_tx);
+        mbar_wait(bars.a_empty(ri.idx), ri.phase ^ 1);
+        mbar_arrive_expect_tx(bars.a_land(ri.idx), stage_tx);
         const uint32_t dst = smem_u32(smem + p.smem_a_off) + (uint32_t)(ri.idx * p.a_stage_bytes);
-        tma_load_5d(dst, &p.tm_x, A_LAND(ri.idx), 0, ci.ti.wi * TW - pw, ci.ti.hi * TH - ph, ci.kc * cpv, ci.ti.b * a.D + ci.din);
+        tma_load_5d(dst, &p.tm_x, bars.a_land(ri.idx), 0, ci.ti.wi * TW - pw, ci.ti.hi * TH - ph, ci.kc * cpv, ci.ti.b * a.D + ci.din);
         ri.advance(); ci.next(tw, p);
       }
     } else {
-    mbar_wait(A_EMPTY(ri.idx), ri.phase ^ 1, 1);
+    mbar_wait(bars.a_empty(ri.idx), ri.phase ^ 1);
     const uint32_t dst = smem_a + (uint32_t)(ri.idx * p.a_stage_bytes) + (uint32_t)v0 * 16u;
     const int hb = ci.ti.hi * TH - ph, wb = ci.ti.wi * TW - pw;
     const bool interior = hb >= 0 && wb >= 0 && hb + p.HALO_H <= a.H && wb + p.HALO_W <= a.W;
@@ -214,15 +206,15 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
   };
 
   const float slope = act_slope(act);
+  const bool relu = act == B200SEG_ACT_RELU;
   float sc[8], sf[8];                              // x*sc + sf == (x - mean) * rstd for this thread's 8 channels
   int norm_key = -1;                               // (b, kc) the constants belong to
 #pragma unroll
   for (int i = 0; i < P; ++i) { if (ci.valid(tw)) issue(); if constexpr (!TMA) cp_async_commit(); }
   while (cd.valid(tw)) {
-    if constexpr (TMA) mbar_wait(A_LAND(rd.idx), rd.phase, 7);
-    else { TC_PROF(11); cp_async_wait<P - 1>(); }      // this thread's copies of the oldest stage have landed
+    if constexpr (TMA) mbar_wait(bars.a_land(rd.idx), rd.phase);
+    else cp_async_wait<P - 1>();      // this thread's copies of the oldest stage have landed
     if (xform && active) {
-      TC_PROF(12);
       const int key = cd.ti.b * p.NKC + cd.kc;
       if (key != norm_key) {
         norm_key = key;
@@ -250,9 +242,14 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
           if constexpr (TMA) raw[u] = make_uint4(0, 0, 0, 0);
           if (ok[u]) raw[u] = *reinterpret_cast<const uint4*>(chunk(i));
         }
-        if constexpr (TMA) {
-          if (act == B200SEG_ACT_RELU) transform3<true>(raw, sc, sf, slope);
-          else transform3<false>(raw, sc, sf, slope);
+        if constexpr (TMA) {      // one branch per batch: the three chunks' dependency chains interleave
+          if (relu) {
+#pragma unroll
+            for (int u = 0; u < 3; ++u) raw[u] = norm_act8<true>(raw[u], sc, sf, slope);
+          } else {
+#pragma unroll
+            for (int u = 0; u < 3; ++u) raw[u] = norm_act8<false>(raw[u], sc, sf, slope);
+          }
 #pragma unroll
           for (int u = 0; u < 3; ++u)
             if (ok[u]) *reinterpret_cast<uint4*>(chunk(i0 + u)) = raw[u];
@@ -260,26 +257,16 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
 #pragma unroll
           for (int u = 0; u < 3; ++u) {
             if (!ok[u]) continue;
-            __half2* hv = reinterpret_cast<__half2*>(&raw[u]);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              float2 f = __half22float2(hv[j]);
-              f.x = fmaf(f.x, sc[2 * j], sf[2 * j]); f.y = fmaf(f.y, sc[2 * j + 1], sf[2 * j + 1]);
-              if (act) { f.x = act_apply(f.x, act); f.y = act_apply(f.y, act); }
-              hv[j] = __floats2half2_rn(f.x, f.y);
-            }
+            raw[u] = relu ? norm_act8<true>(raw[u], sc, sf, slope) : norm_act8<false>(raw[u], sc, sf, slope);
             *reinterpret_cast<uint4*>(chunk(i0 + u)) = raw[u];
           }
         }
       }
     }
-    {
-      TC_PROF(17);
-      fence_proxy_async();          // generic-proxy / cp.async writes -> visible to the tensor core (async proxy)
-      mbar_arrive(A_FULL(rd.idx));
-    }
-    { TC_PROF(18); rd.advance(); cd.next(tw, p); }
-    if (ci.valid(tw)) { TC_PROF(15); issue(); }
+    fence_proxy_async();          // generic-proxy / cp.async writes -> visible to the tensor core (async proxy)
+    mbar_arrive(bars.a_full(rd.idx));
+    rd.advance(); cd.next(tw, p);
+    if (ci.valid(tw)) issue();
     if constexpr (!TMA) cp_async_commit();
   }
   if constexpr (!TMA) cp_async_wait<0>();
@@ -290,25 +277,23 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
 // conv padding / ragged tiles — and the MMA warpgroups consume the stage straight off the TMA's transaction barrier: no
 // loader instruction touches the data.  (Inputs that need InstanceNorm / activation go through loader_role<P>, whose TMA
 // mode lands the same box and then transforms it in place with the cp.async path's per-thread chunk table.)
-__device__ __forceinline__ void loader_role_tma(const TcParams& p, uint8_t* smem, uint32_t bar0) {
+__device__ __forceinline__ void loader_role_tma(const TcParams& p, uint8_t* smem, const Bars& bars) {
   const ConvArgs& a = p.a;
   const int lt = threadIdx.x - kLoadWarp0 * 32;
   const int ph = a.kh / 2, pw = a.kw / 2;
   const uint32_t smem_a = smem_u32(smem + p.smem_a_off);
-  auto A_EMPTY = [&](int i) { return bar0 + 8u * (uint32_t)(p.SA + i); };
-  auto A_LAND = [&](int i) { return bar0 + 8u * (uint32_t)(2 * p.SA + 2 * p.SB + i); };
   TileWalk tw; tw.init(p);
   const uint32_t stage_tx = (uint32_t)((p.KC / 8) * p.nvox_h * 16);
   auto issue = [&](const StageCursor& c, int slot) {
-    mbar_arrive_expect_tx(A_LAND(slot), stage_tx);
-    tma_load_5d(smem_a + (uint32_t)(slot * p.a_stage_bytes), &p.tm_x, A_LAND(slot), 0, c.ti.wi * TW - pw, c.ti.hi * TH - ph,
+    mbar_arrive_expect_tx(bars.a_land(slot), stage_tx);
+    tma_load_5d(smem_a + (uint32_t)(slot * p.a_stage_bytes), &p.tm_x, bars.a_land(slot), 0, c.ti.wi * TW - pw, c.ti.hi * TH - ph,
                   c.kc * (p.KC / 8), c.ti.b * a.D + c.din);
   };
   if (lt == 0) {
     StageCursor c; c.init(tw, p);
     Ring r; r.init(p.SA);
     for (; c.valid(tw); c.next(tw, p)) {
-      mbar_wait(A_EMPTY(r.idx), r.phase ^ 1, 1);
+      mbar_wait(bars.a_empty(r.idx), r.phase ^ 1);
       issue(c, r.idx);
       r.advance();
     }
@@ -326,13 +311,10 @@ __device__ __forceinline__ void loader_role_tma(const TcParams& p, uint8_t* smem
 // then each warp adds them to y_stats with one fp64 atomic per value.  Every addition before the atomic happens in a
 // fixed order; the order of the fp64 atomics can move only the last fp64 bits of the statistics.
 template <int NT>
-__device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid, uint8_t* smem, uint32_t bar0, const float2* s_gnorm) {
+__device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid, uint8_t* smem, const Bars& bars, const float2* s_gnorm) {
   const ConvArgs& a = p.a;
-  auto A_EMPTY = [&](int i) { return bar0 + 8u * (uint32_t)(p.SA + i); };
-  auto B_FULL = [&](int i) { return bar0 + 8u * (uint32_t)(2 * p.SA + i); };
-  auto B_EMPTY = [&](int i) { return bar0 + 8u * (uint32_t)(2 * p.SA + p.SB + i); };
   // A stage ready: published by the loaders, or (raw input staged by TMA) the TMA's own transaction barrier
-  const uint32_t a_ready0 = (p.use_tma && !(a.x_stats || a.act)) ? bar0 + 8u * (uint32_t)(2 * p.SA + 2 * p.SB) : bar0;
+  const uint32_t a_ready0 = (p.use_tma && !(a.x_stats || a.act)) ? bars.a_land(0) : bars.a_full(0);
   const int warp = tid >> 5, lane = tid & 31;
   const bool signaller = tid == 0;
   const int r0 = 64 * wg + 16 * warp + (lane >> 2);
@@ -371,13 +353,13 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
       ks[k][0] = ks[k][1] = ks[k][2] = ks[k][3] = 0.f;
     }
   };
-  if (resident) mbar_wait(B_FULL(0), 0, 10);
+  if (resident) mbar_wait(bars.b_full(0), 0);
   Ring ra, rb; ra.init(p.SA); rb.init(p.SB);
   int pend_a = -1, pend_b = -1;                                        // slots read only by the group in flight
   auto release = [&]() {
     if (signaller) {
-      if (pend_b >= 0) mbar_arrive(B_EMPTY(pend_b));
-      if (pend_a >= 0) mbar_arrive(A_EMPTY(pend_a));
+      if (pend_b >= 0) mbar_arrive(bars.b_empty(pend_b));
+      if (pend_a >= 0) mbar_arrive(bars.a_empty(pend_a));
     }
     pend_a = -1; pend_b = -1;
   };
@@ -390,7 +372,7 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
       for (int zd = 0; zd < a.kd; ++zd) {
         const int din = tc.d + zd - pd;
         if ((unsigned)din >= (unsigned)a.D) continue;
-        mbar_wait(a_ready0 + 8u * (uint32_t)ra.idx, ra.phase, 9);
+        mbar_wait(a_ready0 + 8u * (uint32_t)ra.idx, ra.phase);
         uint64_t da_row = a_tmpl + (uint64_t)(smem_a16 + (uint32_t)ra.idx * a_stage16);
         uint64_t db_res = b_tmpl + (uint64_t)(smem_b16 + (uint32_t)((tc.ntile * taps_all + zd * taps_hw) * p.NKC + kc) * b_stage16);
         for (int zh = 0; zh < a.kh; ++zh) {
@@ -401,7 +383,7 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
               db = db_res;
               db_res += (uint64_t)res_step;
             } else {
-              mbar_wait(B_FULL(rb.idx), rb.phase, 10);
+              mbar_wait(bars.b_full(rb.idx), rb.phase);
               db = b_tmpl + (uint64_t)(smem_b16 + (uint32_t)rb.idx * b_stage16);
               bslot = rb.idx;
               rb.advance();
@@ -487,21 +469,12 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  TC_PROF(31);
   const ConvArgs& a = p.a;
   // canonical warp index: the shuffle makes it provably warp-uniform, so the role branches below are uniform branches
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const int taps_hw = a.kh * a.kw;
   const int pd = a.kd / 2;
-
-  // barrier block layout (uint64 each): a_full[SA] a_empty[SA] b_full[SB] b_empty[SB] a_land[SA]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.smem_bar_off);
-  const uint32_t bar0 = smem_u32(bars);
-  auto A_FULL = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-  auto A_EMPTY = [&](int i) { return bar0 + 8u * (uint32_t)(p.SA + i); };
-  auto B_FULL = [&](int i) { return bar0 + 8u * (uint32_t)(2 * p.SA + i); };
-  auto B_EMPTY = [&](int i) { return bar0 + 8u * (uint32_t)(2 * p.SA + p.SB + i); };
-  auto A_LAND = [&](int i) { return bar0 + 8u * (uint32_t)(2 * p.SA + 2 * p.SB + i); };   // TMA mode: the stage's box has landed
+  const Bars bars{smem_u32(smem + p.smem_bar_off), p};
 
   float2* s_norm = reinterpret_cast<float2*>(smem + p.smem_norm_off);   // [B][Cin] {mean, rstd}
   float2* s_gnorm = reinterpret_cast<float2*>(smem + p.smem_gnorm_off); // [B][Cout] {mean, rstd} of dgrad_x
@@ -509,8 +482,8 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
 
   // ---- one-time setup
   if (threadIdx.x == 0) {
-    for (int i = 0; i < p.SA; ++i) { mbar_init(A_FULL(i), kLoadThreads); mbar_init(A_EMPTY(i), kConsumerWGs); mbar_init(A_LAND(i), 1); }
-    for (int i = 0; i < p.SB; ++i) { mbar_init(B_FULL(i), 1); mbar_init(B_EMPTY(i), kConsumerWGs); }
+    for (int i = 0; i < p.SA; ++i) { mbar_init(bars.a_full(i), kLoadThreads); mbar_init(bars.a_empty(i), kConsumerWGs); mbar_init(bars.a_land(i), 1); }
+    for (int i = 0; i < p.SB; ++i) { mbar_init(bars.b_full(i), 1); mbar_init(bars.b_empty(i), kConsumerWGs); }
     fence_barrier_init();
   }
   {
@@ -533,10 +506,10 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   if (warp >= kLoadWarp0 && warp < kWgtWarp) {
     // =========================== A LOADERS ===========================
     setmaxnreg_dec<kRegsLoad>();
-    if (p.use_tma && !(a.x_stats || a.act)) loader_role_tma(p, smem, bar0);
-    else if (p.use_tma) loader_role<3, true>(p, smem, s_norm, bar0);
-    else if (p.prefetch >= 3) loader_role<3, false>(p, smem, s_norm, bar0);
-    else loader_role<1, false>(p, smem, s_norm, bar0);
+    if (p.use_tma && !(a.x_stats || a.act)) loader_role_tma(p, smem, bars);
+    else if (p.use_tma) loader_role<3, true>(p, smem, s_norm, bars);
+    else if (p.prefetch >= 3) loader_role<3, false>(p, smem, s_norm, bars);
+    else loader_role<1, false>(p, smem, s_norm, bars);
   } else if (warp >= kWgtWarp) {
     setmaxnreg_dec<kRegsWgt>();
     if (warp == kWgtWarp && lane == 0) {
@@ -546,9 +519,9 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
       if (p.w_resident) {
         // small layers: the whole weight image is loaded once; the consumers index it directly
         const int nblobs = p.NTILES * taps * p.NKC;
-        mbar_arrive_expect_tx(B_FULL(0), (uint32_t)(nblobs * p.b_stage_bytes));
+        mbar_arrive_expect_tx(bars.b_full(0), (uint32_t)(nblobs * p.b_stage_bytes));
         for (int i = 0; i < nblobs; ++i)
-          bulk_g2s(smem_b + i * p.b_stage_bytes, wimg + (int64_t)i * p.b_stage_bytes, (uint32_t)p.b_stage_bytes, B_FULL(0));
+          bulk_g2s(smem_b + i * p.b_stage_bytes, wimg + (int64_t)i * p.b_stage_bytes, (uint32_t)p.b_stage_bytes, bars.b_full(0));
       } else {
         Ring ring; ring.init(p.SB);
         TileWalk tw; tw.init(p); TileIter ti; ti.init(tw);
@@ -560,10 +533,10 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
               if ((unsigned)din >= (unsigned)a.D) continue;
               for (int thw = 0; thw < taps_hw; ++thw) {
                 const int tap = zd * taps_hw + thw;
-                mbar_wait(B_EMPTY(ring.idx), ring.phase ^ 1, 2);
-                mbar_arrive_expect_tx(B_FULL(ring.idx), (uint32_t)p.b_stage_bytes);
+                mbar_wait(bars.b_empty(ring.idx), ring.phase ^ 1);
+                mbar_arrive_expect_tx(bars.b_full(ring.idx), (uint32_t)p.b_stage_bytes);
                 const uint8_t* src = wimg + ((int64_t)(tc.ntile * taps + tap) * p.NKC + kc) * p.b_stage_bytes;
-                bulk_g2s(smem_b + ring.idx * p.b_stage_bytes, src, (uint32_t)p.b_stage_bytes, B_FULL(ring.idx));
+                bulk_g2s(smem_b + ring.idx * p.b_stage_bytes, src, (uint32_t)p.b_stage_bytes, bars.b_full(ring.idx));
                 ring.advance();
               }
             }
@@ -575,22 +548,11 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
     // =========================== MMA + EPILOGUE (warps 0-7) ===========================
     setmaxnreg_inc<kRegsConsumer>();
     const int wg = warp >> 2, tid = threadIdx.x & 127;
-    switch (p.NT) {
-      case 16: consumer_role<16>(p, wg, tid, smem, bar0, s_gnorm); break;
-      case 32: consumer_role<32>(p, wg, tid, smem, bar0, s_gnorm); break;
-      case 48: consumer_role<48>(p, wg, tid, smem, bar0, s_gnorm); break;
-      case 64: consumer_role<64>(p, wg, tid, smem, bar0, s_gnorm); break;
-      case 80: consumer_role<80>(p, wg, tid, smem, bar0, s_gnorm); break;
-      case 96: consumer_role<96>(p, wg, tid, smem, bar0, s_gnorm); break;
-      case 112: consumer_role<112>(p, wg, tid, smem, bar0, s_gnorm); break;
-      default: consumer_role<128>(p, wg, tid, smem, bar0, s_gnorm); break;
-    }
+    dispatch_n(p.NT, [&](auto nt) { consumer_role<decltype(nt)::value>(p, wg, tid, smem, bars, s_gnorm); });
   }
 }
 
 }  // namespace
-
-TC_PROF_ENTRY(b200seg_conv_tc_prof)
 
 bool conv3d_tc_shape_ok(int Cin, int Cout, int kd, int kh, int kw, int dtype) {
   if (dtype != B200SEG_F16) return false;
@@ -623,13 +585,12 @@ int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
   p.HALO_H = TH + a.kh - 1; p.HALO_W = TW + a.kw - 1;
   p.nvox_h = p.HALO_H * p.HALO_W;
   int slots = p.nvox_h; if ((slots & 1) == 0) slots += 1;     // odd number of 16-B slots -> conflict-free plane stride
-  // Operand staging: RAW inputs (every data-gradient launch) are staged by ONE tensor-TMA box per stage and consumed by
-  // the MMA warpgroups straight off the TMA barrier; inputs that need InstanceNorm / activation by a TMA box + in-place
-  // transform while Cin <= 64, by per-thread cp.async copies + transform beyond that (B200SEG_CONV_TMA_ALL=1: TMA for
-  // every layer, B200SEG_CONV_NO_TMA=1: cp.async for every layer).
+  // Operand staging, chosen from the shape alone: RAW inputs (every data-gradient launch) are staged by ONE tensor-TMA
+  // box per stage and consumed by the MMA warpgroups straight off the TMA barrier; inputs that need InstanceNorm /
+  // activation by a TMA box + in-place transform while Cin <= 64 and at least 4 A stages fit (below), by per-thread
+  // cp.async copies + transform otherwise.  When the tensor map cannot be built every input takes the cp.async path.
   const bool raw_input = !a.x_stats && a.act == 0;
-  const bool tma_ok = !getenv("B200SEG_CONV_NO_TMA") && p.nvox_h <= 192;
-  p.use_tma = (tma_ok && (raw_input || a.Cin <= 64 || getenv("B200SEG_CONV_TMA_ALL")) &&
+  p.use_tma = ((raw_input || a.Cin <= 64) &&
                b200seg_make_act_tmap(&p.tm_x, a.x, a.x_ld, a.x_coff, a.Cin, a.B * a.D, a.H, a.W, p.HALO_W, p.HALO_H, p.KC / 8)) ? 1 : 0;
   p.plane_stride = p.use_tma ? p.nvox_h * 16 : slots * 16;    // a TMA box is written densely
   p.a_stage_bytes = (p.KC / 8) * p.plane_stride;
@@ -677,7 +638,6 @@ int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
     B200_CUDA(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  tc_apply_env();
   conv_tc_kernel<<<grid, kThreads, smem_bytes, st>>>(p);
   B200_CHECK_LAUNCH("conv_tc_kernel");
   return B200SEG_OK;

@@ -1,55 +1,17 @@
-// tc_common.cuh — PTX wrappers shared by the tensor-core kernels (conv_tc.cu, wgrad_tc.cu): mbarrier, bulk-TMA,
-// cp.async, SWIZZLE_NONE wgmma matrix descriptors, warpgroup register re-distribution.
+// tc_common.cuh — pieces shared by the tensor-core kernels (conv_tc.cu, wgrad_tc.cu): PTX wrappers for mbarrier,
+// bulk-TMA, cp.async, SWIZZLE_NONE wgmma matrix descriptors and warpgroup register re-distribution; the loaders'
+// normalise + activate of one staged chunk; the run-time N -> consumer template dispatch.
 // sm_90a; every wrapper is a thin inline-asm statement so the SASS shows HGMMA / UBLKCP / UTMALDG / SYNCS.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
-#include <string.h>
+#include <type_traits>
+#include "common.cuh"
 
 namespace tc {
 
 constexpr long long kWaitTimeoutCycles = 4000000000ll;   // ~2 s at 1.9 GHz: a protocol bug traps, it never hangs the GPU
 constexpr uint32_t kSuspendNs = 20000;         // suspend-time hint of a blocked try_wait (the thread is woken on completion)
-// per-TU copy of the hint the kernels actually pass (tuning knob: env B200SEG_SUSPEND_NS, read once by tc_apply_env())
-__constant__ uint32_t c_suspend_ns = kSuspendNs;
-
-// ---- role profiler (compiled only into libb200seg_prof.so with -DB200SEG_TC_PROFILE; read through the
-// b200seg_conv_tc_prof / b200seg_wgrad_tc_prof entry points of that library) ----
-// Lane 0 of every warp adds the cycles it spends inside a TC_PROF(code) scope (and inside every mbar_wait, keyed by
-// the wait site's code) to a per-CTA row; slot 31 = kernel lifetime of thread 0, slots 32+code = scope entry counts.
-#ifdef B200SEG_TC_PROFILE
-constexpr int kProfSlots = 64, kProfRows = 160;
-__device__ unsigned long long g_tc_prof[kProfRows * kProfSlots];
-struct ProfScope {
-  int code; long long t0;
-  __device__ __forceinline__ explicit ProfScope(int c) { code = c; t0 = clock64(); }
-  __device__ __forceinline__ ~ProfScope() {
-    if ((threadIdx.x & 31) == 0 && blockIdx.x < kProfRows) {
-      atomicAdd(&g_tc_prof[blockIdx.x * kProfSlots + (code & 31)], (unsigned long long)(clock64() - t0));
-      atomicAdd(&g_tc_prof[blockIdx.x * kProfSlots + 32 + (code & 31)], 1ull);
-    }
-  }
-};
-#define TC_PROF(code) ProfScope prof_scope_##code(code)
-#define TC_PROF_ENTRY(name) \
-  extern "C" int name(unsigned long long* out, int reset) { \
-    static unsigned long long h[kProfRows * kProfSlots]; \
-    if (cudaMemcpyFromSymbol(h, g_tc_prof, sizeof(h)) != cudaSuccess) return -1; \
-    for (int i = 0; i < kProfSlots; ++i) { out[i] = 0; for (int r = 0; r < kProfRows; ++r) out[i] += h[r * kProfSlots + i]; } \
-    if (reset) { memset(h, 0, sizeof(h)); cudaMemcpyToSymbol(g_tc_prof, h, sizeof(h)); } \
-    return 0; }
-#else
-#define TC_PROF(code)
-#define TC_PROF_ENTRY(name)
-#endif
-
-inline void tc_apply_env() {
-  static bool done = false;
-  if (done) return;
-  done = true;
-  if (const char* e = getenv("B200SEG_SUSPEND_NS")) { const uint32_t v = (uint32_t)atoi(e); cudaMemcpyToSymbol(c_suspend_ns, &v, sizeof(v)); }
-}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -68,26 +30,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       "{\n\t.reg .pred p;\n\t"
       "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
       "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(bar), "r"(parity), "r"(c_suspend_ns) : "memory");
-  return ok != 0;
-}
-// non-blocking probe (no suspend): has the phase with this parity completed?
-__device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
+      : "=r"(ok) : "r"(bar), "r"(parity), "n"(kSuspendNs) : "memory");
   return ok != 0;
 }
 // bounded wait: a protocol bug must surface as a trap (launch failure), never as a hung GPU.  No out-of-line
 // diagnostics: a CALL anywhere in a kernel that uses setmaxnreg makes ptxas keep every role inside the SMALLEST
 // register allotment (measured: the epilogue stayed below R88 and spilled its accumulators), and a call inside the
-// MMA issue loop pushes the loop off the uniform datapath.  `code` only documents the wait site.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int code) {
-  (void)code;
-  TC_PROF(code);
+// MMA issue loop pushes the loop off the uniform datapath.
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
@@ -106,13 +56,6 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
   asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
                ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
 }
 // 16-byte cp.async (SASS: LDGSTS); src_bytes == 0 zero-fills the destination (out-of-volume voxels)
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
@@ -142,5 +85,39 @@ struct Ring {
   __device__ __forceinline__ void init(int n_) { idx = 0; phase = 0; n = n_; }
   __device__ __forceinline__ void advance() { if (++idx == n) { idx = 0; phase ^= 1; } }
 };
+
+// InstanceNorm-normalise + activate one staged 16-byte chunk (8 fp16 channels) in registers: x*sc + sf (== (x - mean)
+// * rstd), the activation, fp16 rounding.  RELU is a template parameter so the activation choice stays out of the
+// per-element code (common.cuh, act_apply_s).  ReLU is fmaxf(h, 0) (NaN -> 0, never -0); LeakyReLU and "none" are
+// h > 0 ? h : slope * h.
+template <bool RELU>
+__device__ __forceinline__ uint4 norm_act8(uint4 raw, const float (&sc)[8], const float (&sf)[8], float slope) {
+  __half2* hv = reinterpret_cast<__half2*>(&raw);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float2 f = __half22float2(hv[j]);
+    f.x = fmaf(f.x, sc[2 * j], sf[2 * j]); f.y = fmaf(f.y, sc[2 * j + 1], sf[2 * j + 1]);
+    if (RELU) { f.x = fmaxf(f.x, 0.f); f.y = fmaxf(f.y, 0.f); }
+    else { f.x = act_apply_s(f.x, slope); f.y = act_apply_s(f.y, slope); }
+    hv[j] = __floats2half2_rn(f.x, f.y);
+  }
+  return raw;
+}
+
+// Calls f(std::integral_constant<int, N>{}) for the run-time GEMM N of a consumer warpgroup (a multiple of 16 up to
+// 128): the one place where an operand width becomes the template argument of consumer_role<N>.
+template <class F>
+__device__ __forceinline__ void dispatch_n(int n, F&& f) {
+  switch (n) {
+    case 16: f(std::integral_constant<int, 16>{}); break;
+    case 32: f(std::integral_constant<int, 32>{}); break;
+    case 48: f(std::integral_constant<int, 48>{}); break;
+    case 64: f(std::integral_constant<int, 64>{}); break;
+    case 80: f(std::integral_constant<int, 80>{}); break;
+    case 96: f(std::integral_constant<int, 96>{}); break;
+    case 112: f(std::integral_constant<int, 112>{}); break;
+    default: f(std::integral_constant<int, 128>{}); break;
+  }
+}
 
 }  // namespace tc

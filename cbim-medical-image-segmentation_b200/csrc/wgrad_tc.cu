@@ -24,10 +24,8 @@
 #include "common.cuh"
 #include "conv_args.h"
 #include "tc_common.cuh"
-#include "tmap.h"
 #include "wgmma.cuh"
 #include <string.h>
-#include <stdlib.h>
 
 namespace {
 
@@ -51,10 +49,14 @@ struct WgParams {
   int NTC, ci_tiles, co_tiles, ngroups, gbase, grem, S;
   int HALO_H, HALO_W, nvox_h, a_plane, dy_plane, a_bytes, dy_bytes, stage_bytes, NS, prefetch;
   int tiles_h, tiles_w, nvt;
-  int use_tma;                             // operand tiles are staged by tensor-TMA boxes (else 16-byte cp.async)
   int smem_bar_off, smem_norm_off;
-  alignas(64) CUtensorMap tm_dy;           // dy  as {8 ch, w, h, plane, b*D+d}
-  alignas(64) CUtensorMap tm_x;            // x   likewise
+};
+
+// barrier block layout (uint64 each): full[NS] (stage staged and transformed) empty[NS] (stage read by both consumers)
+struct Bars {
+  uint32_t bar0; const WgParams& p;
+  __device__ __forceinline__ uint32_t full(int i) const { return bar0 + 8u * (uint32_t)i; }
+  __device__ __forceinline__ uint32_t empty(int i) const { return bar0 + 8u * (uint32_t)(p.NS + i); }
 };
 
 struct Job { int co_tile, ci_tile, zd, grp, tap0, ntaps, s; };
@@ -106,7 +108,7 @@ struct VtCursor {
 };
 
 template <int P>
-__device__ __forceinline__ void wg_loader(const WgParams& p, const Job& job, uint8_t* smem, const float2* s_norm, uint32_t bar0) {
+__device__ __forceinline__ void wg_loader(const WgParams& p, const Job& job, uint8_t* smem, const float2* s_norm, const Bars& bars) {
   const int lt = threadIdx.x - kLoadWarp0 * 32;
   const int ph = p.kh / 2, pw = p.kw / 2, zoff = job.zd - p.kd / 2;
   const int co0 = job.co_tile * MT;
@@ -124,15 +126,15 @@ __device__ __forceinline__ void wg_loader(const WgParams& p, const Job& job, uin
   const int sh_a = vstep_a / p.HALO_W, sw_a = vstep_a % p.HALO_W;
   const int hh0 = v0_a / p.HALO_W, ww0 = v0_a % p.HALO_W;
   const bool xform = (p.x_stats != nullptr) || (p.act != 0);
-  auto FULL = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-  auto EMPTY = [&](int i) { return bar0 + 8u * (uint32_t)(p.NS + i); };
+  const bool relu = p.act == B200SEG_ACT_RELU;
+  const float slope = act_slope(p.act);
   VtWalk vw; vw.init(p);
   VtCursor ci, cd;
   ci.init(vw, p, job.s, zoff); cd.init(vw, p, job.s, zoff);
   Ring ri, rd; ri.init(p.NS); rd.init(p.NS);
 
   auto issue = [&]() {
-    mbar_wait(EMPTY(ri.idx), ri.phase ^ 1, 1);
+    mbar_wait(bars.empty(ri.idx), ri.phase ^ 1);
     const uint32_t sdy = smem_u32(smem + ri.idx * p.stage_bytes);
     const uint32_t sa = sdy + (uint32_t)p.dy_bytes;
     if (act_d) {
@@ -164,9 +166,8 @@ __device__ __forceinline__ void wg_loader(const WgParams& p, const Job& job, uin
 #pragma unroll
   for (int i = 0; i < P; ++i) { if (ci.valid(p)) issue(); cp_async_commit(); }
   while (cd.valid(p)) {
-    { TC_PROF(11); cp_async_wait<P - 1>(); }
+    cp_async_wait<P - 1>();
     if (xform && act_a) {
-      TC_PROF(12);
       uint8_t* sp = smem + rd.idx * p.stage_bytes + p.dy_bytes + c8_a * p.a_plane;
       float sc[8], sf[8];                          // x*sc + sf == (x - mean) * rstd
 #pragma unroll
@@ -174,138 +175,36 @@ __device__ __forceinline__ void wg_loader(const WgParams& p, const Job& job, uin
         const float2 mr = s_norm[cd.b * p.NTC + c8_a * 8 + j];
         sc[j] = mr.y; sf[j] = -mr.x * mr.y;
       }
-      const int act = p.act;
       int hh = hh0, ww = ww0;
 #pragma unroll 2
       for (int v = v0_a; v < p.nvox_h; v += vstep_a) {
         const int h = cd.h0() - ph + hh, w = cd.w0() - pw + ww;
         if ((unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W) {      // padding voxels stay zero
-          uint4 raw = *reinterpret_cast<const uint4*>(sp + v * 16);
-          __half2* hv = reinterpret_cast<__half2*>(&raw);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float2 f = __half22float2(hv[j]);
-            f.x = fmaf(f.x, sc[2 * j], sf[2 * j]); f.y = fmaf(f.y, sc[2 * j + 1], sf[2 * j + 1]);
-            if (act) { f.x = act_apply(f.x, act); f.y = act_apply(f.y, act); }
-            hv[j] = __floats2half2_rn(f.x, f.y);
-          }
-          *reinterpret_cast<uint4*>(sp + v * 16) = raw;
+          uint4* chunk = reinterpret_cast<uint4*>(sp + v * 16);
+          *chunk = relu ? norm_act8<true>(*chunk, sc, sf, slope) : norm_act8<false>(*chunk, sc, sf, slope);
         }
         hh += sh_a; ww += sw_a;
         if (ww >= p.HALO_W) { ww -= p.HALO_W; ++hh; }
       }
     }
     fence_proxy_async();
-    mbar_arrive(FULL(rd.idx));
+    mbar_arrive(bars.full(rd.idx));
     rd.advance(); cd.next(vw, p, zoff);
-    if (ci.valid(p)) { TC_PROF(15); issue(); }
+    if (ci.valid(p)) issue();
     cp_async_commit();
   }
   cp_async_wait<0>();
-}
-
-// ---- TMA staging: one elected loader thread issues two tensor-TMA boxes per stage (dy tile, x halo tile; out-of-volume
-// voxels zero-filled by the TMA unit), as many stages ahead as the ring has free slots.  When the input needs
-// InstanceNorm / activation, all loader threads then transform the landed halo tile in place and publish FULL; raw
-// operands are consumed straight off the TMA's own barrier (LAND).
-__device__ __forceinline__ void wg_loader_tma(const WgParams& p, const Job& job, uint8_t* smem, const float2* s_norm, uint32_t bar0) {
-  const int lt = threadIdx.x - kLoadWarp0 * 32;
-  const int ph = p.kh / 2, pw = p.kw / 2, zoff = job.zd - p.kd / 2;
-  const int co0 = job.co_tile * MT, ci0 = job.ci_tile * p.NTC;
-  const bool xform = (p.x_stats != nullptr) || (p.act != 0);
-  auto FULL = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-  auto EMPTY = [&](int i) { return bar0 + 8u * (uint32_t)(p.NS + i); };
-  auto LAND = [&](int i) { return bar0 + 8u * (uint32_t)(2 * p.NS + i); };
-  VtWalk vw; vw.init(p);
-  const uint32_t stage_tx = (uint32_t)(p.dy_bytes + p.a_bytes);
-  if (!xform) {
-    if (lt == 0) {
-      VtCursor c; c.init(vw, p, job.s, zoff);
-      Ring r; r.init(p.NS);
-      for (; c.valid(p); c.next(vw, p, zoff)) {
-        mbar_wait(EMPTY(r.idx), r.phase ^ 1, 1);
-        const uint32_t sdy = smem_u32(smem + r.idx * p.stage_bytes);
-        mbar_arrive_expect_tx(LAND(r.idx), stage_tx);
-        tma_load_5d(sdy, &p.tm_dy, LAND(r.idx), 0, c.w0(), c.h0(), co0 / 8, c.b * p.D + c.d);
-        tma_load_5d(sdy + (uint32_t)p.dy_bytes, &p.tm_x, LAND(r.idx), 0, c.w0() - pw, c.h0() - ph, ci0 / 8, c.b * p.D + c.din);
-        r.advance();
-      }
-    }
-    return;
-  }
-  const int cpv_a = p.NTC / 8;
-  const int vstep_a = kLoadThreads / cpv_a;
-  const bool act_a = lt < vstep_a * cpv_a;
-  const int c8_a = lt % cpv_a, v0_a = lt / cpv_a;
-  const int sh_a = vstep_a / p.HALO_W, sw_a = vstep_a % p.HALO_W;
-  const int hh0 = v0_a / p.HALO_W, ww0 = v0_a % p.HALO_W;
-  const int act = p.act;
-  VtCursor ci, cd;
-  ci.init(vw, p, job.s, zoff); cd.init(vw, p, job.s, zoff);
-  Ring ri, rd; ri.init(p.NS); rd.init(p.NS);
-  int ahead = 0;
-  float sc[8], sf[8];
-  int norm_b = -1;
-  while (cd.valid(p)) {
-    if (lt == 0) {                 // run ahead as far as the ring has free slots; block only when nothing is in flight
-      while (ci.valid(p) && ahead < p.NS) {
-        if (!mbar_test_wait(EMPTY(ri.idx), ri.phase ^ 1)) { if (ahead > 0) break; mbar_wait(EMPTY(ri.idx), ri.phase ^ 1, 1); }
-        const uint32_t sdy = smem_u32(smem + ri.idx * p.stage_bytes);
-        mbar_arrive_expect_tx(LAND(ri.idx), stage_tx);
-        tma_load_5d(sdy, &p.tm_dy, LAND(ri.idx), 0, ci.w0(), ci.h0(), co0 / 8, ci.b * p.D + ci.d);
-        tma_load_5d(sdy + (uint32_t)p.dy_bytes, &p.tm_x, LAND(ri.idx), 0, ci.w0() - pw, ci.h0() - ph, ci0 / 8, ci.b * p.D + ci.din);
-        ri.advance(); ci.next(vw, p, zoff); ++ahead;
-      }
-    }
-    mbar_wait(LAND(rd.idx), rd.phase, 7);
-    if (act_a) {
-      if (cd.b != norm_b) {
-        norm_b = cd.b;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float2 mr = s_norm[cd.b * p.NTC + c8_a * 8 + j];
-          sc[j] = mr.y; sf[j] = -mr.x * mr.y;
-        }
-      }
-      uint8_t* sp = smem + rd.idx * p.stage_bytes + p.dy_bytes + c8_a * p.a_plane;
-      int hh = hh0, ww = ww0;
-#pragma unroll 2
-      for (int v = v0_a; v < p.nvox_h; v += vstep_a) {
-        const int h = cd.h0() - ph + hh, w = cd.w0() - pw + ww;
-        if ((unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W) {      // zero-filled padding voxels stay zero
-          uint4 raw = *reinterpret_cast<const uint4*>(sp + v * 16);
-          __half2* hv = reinterpret_cast<__half2*>(&raw);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float2 f = __half22float2(hv[j]);
-            f.x = act_apply(fmaf(f.x, sc[2 * j], sf[2 * j]), act); f.y = act_apply(fmaf(f.y, sc[2 * j + 1], sf[2 * j + 1]), act);
-            hv[j] = __floats2half2_rn(f.x, f.y);
-          }
-          *reinterpret_cast<uint4*>(sp + v * 16) = raw;
-        }
-        hh += sh_a; ww += sw_a;
-        if (ww >= p.HALO_W) { ww -= p.HALO_W; ++hh; }
-      }
-    }
-    fence_proxy_async();
-    mbar_arrive(FULL(rd.idx));
-    rd.advance(); cd.next(vw, p, zoff);
-    if (lt == 0) --ahead;
-  }
 }
 
 // ---- MMA warpgroup g: output channels co0 + 64g .. +63 of the M tile, every tap of the job's group.  Per voxel tile one
 // wgmma group (ntaps x 8 instructions m64 x NTC x 16) is committed; the stage the group before it read is then handed
 // back.  After the last tile the accumulators are added into dW (thread: rows 16w + l/4 (+8), column pairs 8j + 2(l%4)).
 template <int NTC>
-__device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job, int wg, int tid, uint8_t* smem, uint32_t bar0) {
+__device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job, int wg, int tid, uint8_t* smem, const Bars& bars) {
   constexpr int GMAX = kMaxCols / NTC < 9 ? kMaxCols / NTC : 9;
   const int zoff = job.zd - p.kd / 2;
   const int co0 = job.co_tile * MT, co_real = min(MT, p.Cout - co0), ci0 = job.ci_tile * NTC;
   const bool live = wg * 64 < co_real;                    // warpgroup-uniform: this half of the M tile holds real channels
-  auto EMPTY = [&](int i) { return bar0 + 8u * (uint32_t)(p.NS + i); };
-  // operands ready: FULL (published by the loaders) or, for raw operands staged by TMA, the TMA's own barrier
-  const uint32_t ready0 = (p.use_tma && !(p.x_stats || p.act)) ? bar0 + 8u * (uint32_t)(2 * p.NS) : bar0;
   // dy^T as the A operand: MN-major (lbo = next 8 voxels, sbo = next channel plane); x halo tile as the B operand:
   // MN-major (lbo = next halo row of voxels, sbo = next channel plane), a tap = start shifted by whole voxel slots
   const uint64_t dy_tmpl = make_desc(0, 128u, (uint32_t)p.dy_plane);
@@ -325,7 +224,7 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
   int pend = -1;
   uint32_t accumulate = 0;
   for (; c.valid(p); c.next(vw, p, zoff)) {
-    mbar_wait(ready0 + 8u * (uint32_t)r.idx, r.phase, 9);
+    mbar_wait(bars.full(r.idx), r.phase);
     if (live) {
       const uint64_t da0 = dy_tmpl + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy_wg16);
       uint64_t db_tap = a_tmpl + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy16 + (uint32_t)(zh0 * HALO_W + zw0));
@@ -349,7 +248,7 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
 #pragma unroll
       for (int g = 0; g < GMAX; ++g) wgmma_fence_operands(acc[g]);
     }
-    if (pend >= 0 && tid == 0) mbar_arrive(EMPTY(pend));
+    if (pend >= 0 && tid == 0) mbar_arrive(bars.empty(pend));
     pend = r.idx;
     accumulate = 1;
     r.advance();
@@ -359,7 +258,7 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
 #pragma unroll
     for (int g = 0; g < GMAX; ++g) wgmma_fence_operands(acc[g]);
   }
-  if (pend >= 0 && tid == 0) mbar_arrive(EMPTY(pend));
+  if (pend >= 0 && tid == 0) mbar_arrive(bars.empty(pend));
   if (!live) return;
   // S == 1: this CTA is the only contributor of its dW elements, one add each.  S > 1: the partial tile goes to its own
   // slice of the split-K buffer (zeros when the CTA owned no voxel tile) and add_slices sums the slices in order,
@@ -390,20 +289,15 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
 __global__ void __launch_bounds__(kThreads, 1)
 wgrad_tc_kernel(const __grid_constant__ WgParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  TC_PROF(31);
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const Job job = decode_job(p, blockIdx.x);
   const int ci0 = job.ci_tile * p.NTC;
 
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.smem_bar_off);
-  const uint32_t bar0 = smem_u32(bars);
-  auto FULL = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-  auto EMPTY = [&](int i) { return bar0 + 8u * (uint32_t)(p.NS + i); };
-  auto LAND = [&](int i) { return bar0 + 8u * (uint32_t)(2 * p.NS + i); };         // TMA mode: the stage's boxes have landed
+  const Bars bars{smem_u32(smem + p.smem_bar_off), p};
   float2* s_norm = reinterpret_cast<float2*>(smem + p.smem_norm_off);     // [B][NTC] {mean, rstd} of this job's channels
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < p.NS; ++i) { mbar_init(FULL(i), kLoadThreads); mbar_init(EMPTY(i), kConsumerWGs); mbar_init(LAND(i), 1); }
+    for (int i = 0; i < p.NS; ++i) { mbar_init(bars.full(i), kLoadThreads); mbar_init(bars.empty(i), kConsumerWGs); }
     fence_barrier_init();
   }
   {
@@ -419,23 +313,13 @@ wgrad_tc_kernel(const __grid_constant__ WgParams p) {
 
   if (warp >= kLoadWarp0) {
     // =========================== LOADERS ===========================
-    if (p.use_tma) wg_loader_tma(p, job, smem, s_norm, bar0);
-    else if (p.prefetch >= 3) wg_loader<3>(p, job, smem, s_norm, bar0);
-    else if (p.prefetch == 2) wg_loader<2>(p, job, smem, s_norm, bar0);
-    else wg_loader<1>(p, job, smem, s_norm, bar0);
+    if (p.prefetch >= 3) wg_loader<3>(p, job, smem, s_norm, bars);
+    else if (p.prefetch == 2) wg_loader<2>(p, job, smem, s_norm, bars);
+    else wg_loader<1>(p, job, smem, s_norm, bars);
   } else {
     // =========================== MMA + EPILOGUE ===========================
     const int wg = warp >> 2, tid = threadIdx.x & 127;
-    switch (p.NTC) {
-      case 16: consumer_role<16>(p, job, wg, tid, smem, bar0); break;
-      case 32: consumer_role<32>(p, job, wg, tid, smem, bar0); break;
-      case 48: consumer_role<48>(p, job, wg, tid, smem, bar0); break;
-      case 64: consumer_role<64>(p, job, wg, tid, smem, bar0); break;
-      case 80: consumer_role<80>(p, job, wg, tid, smem, bar0); break;
-      case 96: consumer_role<96>(p, job, wg, tid, smem, bar0); break;
-      case 112: consumer_role<112>(p, job, wg, tid, smem, bar0); break;
-      default: consumer_role<128>(p, job, wg, tid, smem, bar0); break;
-    }
+    dispatch_n(p.NTC, [&](auto ntc) { consumer_role<decltype(ntc)::value>(p, job, wg, tid, smem, bars); });
   }
 }
 
@@ -443,16 +327,14 @@ wgrad_tc_kernel(const __grid_constant__ WgParams p) {
 // tile), else the whole Cin up to 128, else the largest of 128 / 96 / 64 / 48 / 32 / 16 dividing it.
 int pick_ntc(int Cin) {
   if (Cin % 16) return 0;
-  int cap = 128;
-  if (const char* e = getenv("B200SEG_WGRAD_NTC_MAX")) { const int v = atoi(e); if (v >= 16) cap = v; }   // tuning knob
-  if (Cin % 128 == 0 && cap >= 64) return 64;
-  if (Cin <= cap) return Cin;
+  if (Cin % 128 == 0) return 64;
+  if (Cin <= 128) return Cin;
   const int c[] = {128, 96, 64, 48, 32, 16};
-  for (int v : c) if (v <= cap && Cin % v == 0) return v;
+  for (int v : c) if (Cin % v == 0) return v;
   return 0;
 }
 
-bool fill_params(const WgradArgs& a, WgParams& p, bool tma = false) {
+bool fill_params(const WgradArgs& a, WgParams& p) {
   memset(&p, 0, sizeof(p));
   p.B = a.B; p.D = a.D; p.H = a.H; p.W = a.W; p.Cin = a.Cin; p.Cout = a.Cout; p.kd = a.kd; p.kh = a.kh; p.kw = a.kw;
   p.NTC = pick_ntc(a.Cin);
@@ -466,9 +348,8 @@ bool fill_params(const WgradArgs& a, WgParams& p, bool tma = false) {
   p.gbase = taps_hw / p.ngroups; p.grem = taps_hw % p.ngroups;
   p.HALO_H = TH + a.kh - 1; p.HALO_W = TW + a.kw - 1; p.nvox_h = p.HALO_H * p.HALO_W;
   int slots = p.nvox_h; if ((slots & 1) == 0) ++slots;
-  p.use_tma = tma ? 1 : 0;                                     // (dense planes: a TMA box is written contiguously)
-  p.a_plane = p.use_tma ? p.nvox_h * 16 : slots * 16;
-  p.dy_plane = p.use_tma ? TH * TW * 16 : (TH * TW + 1) * 16;
+  p.a_plane = slots * 16;
+  p.dy_plane = (TH * TW + 1) * 16;
   p.a_bytes = (p.NTC / 8) * p.a_plane; p.a_bytes = (p.a_bytes + 127) / 128 * 128;
   // only the real output-channel planes of the widest M tile are staged; the descriptors' 8-plane footprint beyond
   // them falls on the `a` tile / the next stage / the tail slack (allocated below), whose values feed rows never read
@@ -490,15 +371,13 @@ bool fill_params(const WgradArgs& a, WgParams& p, bool tma = false) {
   p.S = S;
   int off = p.NS * p.stage_bytes + 16 * p.dy_plane;       // + slack for the 16-plane descriptor footprint
   off = (off + 15) / 16 * 16;
-  p.smem_bar_off = off; off += 3 * p.NS * 8;
+  p.smem_bar_off = off; off += 2 * p.NS * 8;
   off = (off + 15) / 16 * 16;
   p.smem_norm_off = off;
   return true;
 }
 
 }  // namespace
-
-TC_PROF_ENTRY(b200seg_wgrad_tc_prof)
 
 bool conv3d_wgrad_tc_supported(const WgradArgs& a, int dtype) {
   if (dtype != B200SEG_F16) return false;
@@ -523,25 +402,11 @@ int conv3d_wgrad_tc(const WgradArgs& a, int dtype, void* workspace, size_t ws_by
   const size_t need = conv3d_wgrad_tc_workspace(a);
   if (need && (!workspace || ws_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 15))) return B200SEG_EINVAL;
   WgParams p;
-  // tensor-TMA staging of both operands is opt-in (B200SEG_WGRAD_TMA=1); by default 256 loader threads stage them
-  // with 16-byte cp.async copies
-  const bool want_tma = getenv("B200SEG_WGRAD_TMA") != nullptr;
-  fill_params(a, p, want_tma);
+  fill_params(a, p);
   p.x = reinterpret_cast<const __half*>(a.x); p.x_ld = a.x_ld; p.x_coff = a.x_coff;
   p.x_stats = a.x_stats; p.eps = a.eps; p.act = a.act;
   p.dy = reinterpret_cast<const __half*>(a.dy); p.dy_ld = a.dy_ld; p.dy_coff = a.dy_coff;
   p.dw = a.dw;
-  if (p.use_tma) {
-    const int co_planes = (a.Cout < MT ? a.Cout : MT) / 8;
-    if (!b200seg_make_act_tmap(&p.tm_dy, a.dy, a.dy_ld, a.dy_coff, a.Cout, a.B * a.D, a.H, a.W, TW, TH, co_planes) ||
-        !b200seg_make_act_tmap(&p.tm_x, a.x, a.x_ld, a.x_coff, a.Cin, a.B * a.D, a.H, a.W, p.HALO_W, p.HALO_H, p.NTC / 8)) {
-      fill_params(a, p, false);               // tensor maps unavailable: fall back to the cp.async staging layout
-      p.x = reinterpret_cast<const __half*>(a.x); p.x_ld = a.x_ld; p.x_coff = a.x_coff;
-      p.x_stats = a.x_stats; p.eps = a.eps; p.act = a.act;
-      p.dy = reinterpret_cast<const __half*>(a.dy); p.dy_ld = a.dy_ld; p.dy_coff = a.dy_coff;
-      p.dw = a.dw;
-    }
-  }
   const int64_t jobs = (int64_t)p.co_tiles * p.ci_tiles * a.kd * p.ngroups;
   const int smem_bytes = p.smem_norm_off + a.B * p.NTC * 8 + 64;
   static thread_local bool attr_set = false;
@@ -551,7 +416,6 @@ int conv3d_wgrad_tc(const WgradArgs& a, int dtype, void* workspace, size_t ws_by
   }
   const int grid = (int)(jobs * p.S);
   p.part = reinterpret_cast<float*>(workspace);
-  tc_apply_env();
   wgrad_tc_kernel<<<grid, kThreads, smem_bytes, st>>>(p);
   B200_CHECK_LAUNCH("wgrad_tc_kernel");
   if (p.S > 1) {

@@ -23,6 +23,7 @@ CASES = [
     (32, 32, (1, 3, 3), (1, 8, 64, 64), "normres"),
     (128, 128, (3, 3, 3), (1, 16, 64, 64), "normres"),   # many tiles per CTA, streamed weights
     (64, 64, (1, 3, 3), (1, 16, 128, 128), "normres"),   # resident weights, many tiles
+    (64, 32, (3, 3, 3), (64, 1, 16, 8), "norm"),          # large B*Cin tables leave 3 A stages: 1-stage cp.async loader
 ]
 
 
