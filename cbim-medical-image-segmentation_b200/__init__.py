@@ -14,7 +14,8 @@ from .medformer import MedFormer
 from .swin_unetr import SwinUNETR
 from .unet3d import UNet
 from .unetpp import UNetPlusPlus
+from .unetr import UNETR
 
-__all__ = ["augmentation", "get_model", "UNet", "MedFormer", "SwinUNETR", "UNetPlusPlus", "AttentionUNet", "DiceLoss", "DiceCELoss", "CrossEntropyLoss", "B200SegError",
+__all__ = ["augmentation", "get_model", "UNet", "MedFormer", "SwinUNETR", "UNETR", "UNetPlusPlus", "AttentionUNet", "DiceLoss", "DiceCELoss", "CrossEntropyLoss", "B200SegError",
            "EXPORTED_SYMBOLS", "LIB_PATH", "get_inference", "inference_sliding_window", "inference_whole_image",
            "calculate_dice", "calculate_dice_split"]

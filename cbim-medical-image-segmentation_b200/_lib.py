@@ -65,6 +65,8 @@ _PROTOS = {
     "b200seg_window_attn_fwd": [P, P, P, P, P, I, I, I, I, I, I, P, P, I, P],
     "b200seg_window_attn_bwd": [P, P, P, P, P, P, P, P, P, P, I, I, I, I, I, I, P, P, I, P],
     "b200seg_swin_merge": [P, P, I, I, I, I, I, I, I, I, P],
+    "b200seg_attention_fwd": [P, P, P, I, I, I, I, I, P],
+    "b200seg_attention_bwd": [P, P, P, P, P, P, I, I, I, I, I, P],
     "b200seg_optim_chunk_elems": [],
     "b200seg_grads_nonfinite": [P, P, I, P, P],
     "b200seg_adamw_ema_step": [P, P, I, F, F, F, F, F, F, P, P, P, P],
@@ -121,7 +123,7 @@ def check(rc, what):
 
 
 # kernels launched per entry point (dice fwd = reduce + finalize; its memset is not ours)
-_KERNELS = {"b200seg_dice_ce_fwd": 2, "b200seg_biattn_fwd": 2, "b200seg_window_attn_bwd": 2, "b200seg_adamw_ema_step": 2, "b200seg_biattn_bwd": 2,
+_KERNELS = {"b200seg_dice_ce_fwd": 2, "b200seg_biattn_fwd": 2, "b200seg_window_attn_bwd": 2, "b200seg_attention_bwd": 3, "b200seg_adamw_ema_step": 2, "b200seg_biattn_bwd": 2,
             "b200seg_mapgen_fwd": 2, "b200seg_attn_gate_fwd": 2, "b200seg_attn_gate_bwd": 2}
 launch_count = 0
 

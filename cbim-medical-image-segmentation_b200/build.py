@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200seg.so")
-SOURCES = ["api.cu", "dice_ce.cu", "instnorm.cu", "pool_upsample.cu", "conv_direct.cu", "conv_tc.cu", "wgrad_tc.cu", "small_conv.cu", "biattn.cu", "dwconv.cu", "medformer_small.cu", "swin.cu", "swin_mma.cu", "optim.cu", "inference.cu", "augment.cu", "attn_gate.cu"]
+SOURCES = ["api.cu", "dice_ce.cu", "instnorm.cu", "pool_upsample.cu", "conv_direct.cu", "conv_tc.cu", "wgrad_tc.cu", "small_conv.cu", "biattn.cu", "dwconv.cu", "medformer_small.cu", "swin.cu", "swin_mma.cu", "optim.cu", "inference.cu", "augment.cu", "attn_gate.cu", "attention.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC"]

@@ -36,6 +36,10 @@ def get_model(args, pretrain=False):
             if getattr(args, 'pretrain', False) or pretrain:
                 raise ValueError('No pretrain model available')   # model/utils.py:113-115 loads a site-local file
             return SwinUNETR(args.window_size, args.in_chan, args.classes, feature_size=args.base_chan)   # :111
+        if args.model == 'unetr':
+            from .unetr import UNETR                        # no pretrain check, as in the reference
+            return UNETR(args.in_chan, args.classes, args.training_size, feature_size=16, hidden_size=768, mlp_dim=3072,
+                         num_heads=12, pos_embed='perceptron', norm_name='instance', res_block=True)
         raise ValueError("model %r (3d) is not implemented by the H100 path" % (args.model,))
     if args.dimension == '2d':
         raise ValueError("2d models are outside the GPU hot path (SURVEY.md §2); use the reference")

@@ -386,6 +386,23 @@ int b200seg_swin_merge(const void* x, void* y, int B, int D, int H, int W, int C
                        int reverse, int v2, int dtype, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * UNETR operators (model/dim3/unetr.py; its ViT encoder is monai 1.1.0's).
+ *
+ * attention: the core of monai's SABlock between its qkv and out_proj Linears,
+ *   out = softmax(q k^T * dim_head^-0.5) v per (batch, head) over all L tokens.
+ *   qkv [B][L][3*heads*dim_head], channel which*inner + h*dim_head + d (q, k, v);
+ *   out [B][L][heads*dim_head], channel h*dim_head + d.  lse: fp32 [B][heads][L]
+ *   row log-sum-exp written by fwd and read by bwd; delta: fp32 [B][heads][L]
+ *   scratch of bwd.  bwd writes every element of dqkv (same layout as qkv) and is
+ *   deterministic.  dim_head must be 64 (else B200SEG_EUNSUPPORTED), any L >= 1;
+ *   qkv / out / dout / dqkv 16-byte aligned.
+ * ------------------------------------------------------------------------- */
+int b200seg_attention_fwd(const void* qkv, void* out, float* lse, int B, int L, int heads, int dim_head,
+                          int dtype, void* stream);
+int b200seg_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* delta,
+                          void* dqkv, int B, int L, int heads, int dim_head, int dtype, void* stream);
+
+/* ---------------------------------------------------------------------------
  * Optimiser tail (SURVEY.md 8f.1): GradScaler non-finite check + unscale, AdamW
  * (training/utils.py:8-14, eps 1e-5) and the EMA update (training/utils.py:98-105,
  * ema_alpha = this iteration's min(1 - 1/(iter+1), cap), computed by the caller) as
