@@ -40,7 +40,8 @@ extern "C" int b200seg_check_device(void) {
 }
 
 extern "C" int b200seg_conv3d_algo(int Cin, int Cout, int kd, int kh, int kw, int dtype, int B) {
-  // (outputs wider than 2048 channels per batch run on the tensor cores only without fused statistics, conv_tc.cu)
+  // the same batch limits as conv3d_fwd_tc_supported, so every shape routed here runs on the tensor cores with or
+  // without fused statistics / dgrad mode
   if (conv3d_tc_shape_ok(Cin, Cout, kd, kh, kw, dtype) && B * Cin <= 4096 && B * Cout <= 8192) return B200SEG_ALGO_TC;
   return B200SEG_ALGO_DIRECT;
 }
