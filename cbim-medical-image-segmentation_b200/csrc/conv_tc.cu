@@ -310,7 +310,9 @@ __device__ __forceinline__ void loader_role_tma(const TcParams& p, uint8_t* smem
 // and kept in registers (lane l keeps the groups j with j % 8 == l / 4) while consecutive tiles share a (batch, N tile);
 // then each warp adds them to y_stats with one fp64 atomic per value.  Every addition before the atomic happens in a
 // fixed order; the order of the fp64 atomics can move only the last fp64 bits of the statistics.
-template <int NT>
+// KSTEPS = KC / 16 is a template argument so that a tap's group is straight-line code: with a run-time trip count the
+// unrolled loop and its remainder made ptxas move accumulators between the MMAs and serialise them (C7519).
+template <int NT, int KSTEPS>
 __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid, uint8_t* smem, const Bars& bars, const float2* s_gnorm) {
   const ConvArgs& a = p.a;
   // A stage ready: published by the loaders, or (raw input staged by TMA) the TMA's own transaction barrier
@@ -320,7 +322,6 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
   const int r0 = 64 * wg + 16 * warp + (lane >> 2);
   const int hl0 = r0 >> 3, wl = r0 & 7;
   const int taps_hw = a.kh * a.kw, pd = a.kd / 2;
-  const int ksteps = p.KC / 16;
   // A: plane image = K-major no-swizzle core matrices (LBO = plane, SBO = one halo row of 16-byte slots)
   const uint64_t a_tmpl = make_desc(0, (uint32_t)p.plane_stride, (uint32_t)p.HALO_W * 16u);
   const uint64_t b_tmpl = make_desc(0, (uint32_t)NT * 16u, 128u);
@@ -391,11 +392,10 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
             const uint64_t da = da_row + (uint64_t)((uint32_t)zh * a_rowstep + (uint32_t)zw);
             wgmma_fence_operands(acc);
             wgmma_fence();
-#pragma unroll 4
-            for (int j = 0; j < ksteps; ++j) {
-              Wgmma<NT, 0, 0>::mma(acc, da + (uint64_t)((uint32_t)j * a_kstep), db + (uint64_t)((uint32_t)j * b_kstep), accumulate);
-              accumulate = 1;
-            }
+#pragma unroll
+            for (int j = 0; j < KSTEPS; ++j)
+              Wgmma<NT, 0, 0>::mma(acc, da + (uint64_t)((uint32_t)j * a_kstep), db + (uint64_t)((uint32_t)j * b_kstep), accumulate | (uint32_t)(j > 0));
+            accumulate = 1;
             wgmma_commit();
             wgmma_wait<1>();                       // the previous group has retired: its slots are free
             wgmma_fence_operands(acc);
@@ -466,6 +466,9 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
 }
 
 // ------------------------------------------------------------------ the kernel
+// One instantiation per (NT, KC / 16) that tc_pick_nt / tc_pick_kc can produce, so each gets its own register
+// allocation instead of sharing the worst case of every tile width.
+template <int NT, int KSTEPS>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -548,8 +551,31 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
     // =========================== MMA + EPILOGUE (warps 0-7) ===========================
     setmaxnreg_inc<kRegsConsumer>();
     const int wg = warp >> 2, tid = threadIdx.x & 127;
-    dispatch_n(p.NT, [&](auto nt) { consumer_role<decltype(nt)::value>(p, wg, tid, smem, bars, s_gnorm); });
+    consumer_role<NT, KSTEPS>(p, wg, tid, smem, bars, s_gnorm);
   }
+}
+
+// KC / 16 for KC in {16, 32, 48, 64} (tc_pick_kc) as a compile-time constant
+template <class F>
+void dispatch_ksteps(int ksteps, F&& f) {
+  switch (ksteps) {
+    case 1: f(std::integral_constant<int, 1>{}); break;
+    case 2: f(std::integral_constant<int, 2>{}); break;
+    case 3: f(std::integral_constant<int, 3>{}); break;
+    default: f(std::integral_constant<int, 4>{}); break;
+  }
+}
+
+template <int NT, int KSTEPS>
+int launch_conv_tc(const TcParams& p, int grid, int smem_bytes, cudaStream_t st) {
+  static thread_local bool attr_set = false;
+  if (!attr_set) {
+    B200_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT, KSTEPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_set = true;
+  }
+  conv_tc_kernel<NT, KSTEPS><<<grid, kThreads, smem_bytes, st>>>(p);
+  B200_CHECK_LAUNCH("conv_tc_kernel");
+  return B200SEG_OK;
 }
 
 }  // namespace
@@ -634,12 +660,9 @@ int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
   p.smem_gnorm_off = off; off += gnorm_bytes;
   const int smem_bytes = off + 1024;       // slack for the 1024-B alignment of the dynamic segment
   int grid = p.n_tiles < B200SEG_NUM_SMS ? p.n_tiles : B200SEG_NUM_SMS;
-  static thread_local bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  conv_tc_kernel<<<grid, kThreads, smem_bytes, st>>>(p);
-  B200_CHECK_LAUNCH("conv_tc_kernel");
-  return B200SEG_OK;
+  int rc = B200SEG_OK;
+  dispatch_n(p.NT, [&](auto nt) {
+    dispatch_ksteps(p.KC / 16, [&](auto ks) { rc = launch_conv_tc<decltype(nt)::value, decltype(ks)::value>(p, grid, smem_bytes, st); });
+  });
+  return rc;
 }

@@ -105,9 +105,11 @@ __device__ __forceinline__ uint4 norm_act8(uint4 raw, const float (&sc)[8], cons
 }
 
 // Calls f(std::integral_constant<int, N>{}) for the run-time GEMM N of a consumer warpgroup (a multiple of 16 up to
-// 128): the one place where an operand width becomes the template argument of consumer_role<N>.
+// 128): the one place where an operand width becomes a template argument (of a kernel on the host, of a role on the
+// device).  The caller's lambda is host-only or device-only; the check is disabled so neither side warns about the other.
+#pragma nv_exec_check_disable
 template <class F>
-__device__ __forceinline__ void dispatch_n(int n, F&& f) {
+__host__ __device__ __forceinline__ void dispatch_n(int n, F&& f) {
   switch (n) {
     case 16: f(std::integral_constant<int, 16>{}); break;
     case 32: f(std::integral_constant<int, 32>{}); break;

@@ -38,6 +38,10 @@ constexpr int kLoadThreads = 256;           // all loader warps cooperate on eve
 constexpr int kThreads = 16 * 32;   // 512
 constexpr int MT = 128;                    // output-channel tile (GEMM M)
 constexpr int kMaxCols = 192;              // accumulator columns per job (taps x Cin tile): 96 fp32 registers per thread
+// Registers per thread after the role dispatch, inside the CTA's pool of 512 x 128: the consumer warpgroups hold up to
+// 96 accumulators plus descriptors and epilogue addresses, the loaders' cp.async + transform loop needs far fewer.
+constexpr int kRegsLaunch = 128, kRegsConsumer = 152, kRegsLoad = 104;
+static_assert(2 * 128 * kRegsConsumer + 2 * 128 * kRegsLoad <= kThreads * kRegsLaunch, "register split exceeds the CTA pool");
 
 struct WgParams {
   const __half* x; int x_ld, x_coff;       // raw input; normalised + activated on the fly when x_stats / act
@@ -196,15 +200,41 @@ __device__ __forceinline__ void wg_loader(const WgParams& p, const Job& job, uin
   cp_async_wait<0>();
 }
 
-// ---- MMA warpgroup g: output channels co0 + 64g .. +63 of the M tile, every tap of the job's group.  Per voxel tile one
-// wgmma group (ntaps x 8 instructions m64 x NTC x 16) is committed; the stage the group before it read is then handed
-// back.  After the last tile the accumulators are added into dW (thread: rows 16w + l/4 (+8), column pairs 8j + 2(l%4)).
-template <int NTC>
+// most taps one job's group can have at Cin tile NTC (fill_params: G = min(kMaxCols / NTC, kh * kw), kh, kw <= 3)
+__host__ __device__ constexpr int max_taps(int ntc) { return kMaxCols / ntc < 9 ? kMaxCols / ntc : 9; }
+
+// Calls f(std::integral_constant<int, G>{}) for the job's run-time tap count n, G0 <= n <= GMAX.
+template <int G, int GMAX, class F>
+__device__ __forceinline__ void dispatch_taps(int n, F&& f) {
+  if constexpr (G < GMAX) {
+    if (n != G) { dispatch_taps<G + 1, GMAX>(n, f); return; }
+  }
+  f(std::integral_constant<int, G>{});
+}
+
+// ---- a consumer warpgroup whose 64 rows of the M tile hold no real output channel (Cout <= 64): it issues no MMA and
+// holds no accumulator, it only hands each stage back once it has been staged.
+__device__ __forceinline__ void idle_consumer_role(const WgParams& p, const Job& job, int tid, const Bars& bars) {
+  const int zoff = job.zd - p.kd / 2;
+  VtWalk vw; vw.init(p);
+  VtCursor c; c.init(vw, p, job.s, zoff);
+  Ring r; r.init(p.NS);
+  for (; c.valid(p); c.next(vw, p, zoff)) {
+    mbar_wait(bars.full(r.idx), r.phase);
+    if (tid == 0) mbar_arrive(bars.empty(r.idx));
+    r.advance();
+  }
+}
+
+// ---- MMA warpgroup g: output channels co0 + 64g .. +63 of the M tile, the NTAPS taps of the job's group.  Per voxel
+// tile one wgmma group (NTAPS x 8 instructions m64 x NTC x 16) is committed; the stage the group before it read is then
+// handed back.  After the last tile the accumulators are added into dW (thread: rows 16w + l/4 (+8), column pairs
+// 8j + 2(l%4)).  NTAPS is a template argument and the group has no branch: a run-time tap count made ptxas retire every
+// group before the next one could issue (C7517), which undid the one-group-in-flight pipelining.
+template <int NTC, int NTAPS>
 __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job, int wg, int tid, uint8_t* smem, const Bars& bars) {
-  constexpr int GMAX = kMaxCols / NTC < 9 ? kMaxCols / NTC : 9;
   const int zoff = job.zd - p.kd / 2;
   const int co0 = job.co_tile * MT, co_real = min(MT, p.Cout - co0), ci0 = job.ci_tile * NTC;
-  const bool live = wg * 64 < co_real;                    // warpgroup-uniform: this half of the M tile holds real channels
   // dy^T as the A operand: MN-major (lbo = next 8 voxels, sbo = next channel plane); x halo tile as the B operand:
   // MN-major (lbo = next halo row of voxels, sbo = next channel plane), a tap = start shifted by whole voxel slots
   const uint64_t dy_tmpl = make_desc(0, 128u, (uint32_t)p.dy_plane);
@@ -214,9 +244,15 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
   const uint32_t stage16 = (uint32_t)p.stage_bytes >> 4, dy16 = (uint32_t)p.dy_bytes >> 4;
   const uint32_t smem16 = smem_u32(smem) >> 4;
   const uint32_t dy_wg16 = (uint32_t)(wg * 8 * p.dy_plane) >> 4;
-  const int zh0 = job.tap0 / p.kw, zw0 = job.tap0 % p.kw;
-  const int ntaps = job.ntaps, kw = p.kw, HALO_W = p.HALO_W;
-  float acc[GMAX][NTC / 2];
+  // start of each tap's B operand in the staged halo tile, in 16-byte voxel slots: taps run along w, then wrap to the
+  // next halo row
+  uint32_t tap_off[NTAPS];
+#pragma unroll
+  for (int g = 0; g < NTAPS; ++g) {
+    const int t = job.tap0 + g;
+    tap_off[g] = (uint32_t)((t / p.kw) * p.HALO_W + t % p.kw);
+  }
+  float acc[NTAPS][NTC / 2];
   VtWalk vw; vw.init(p);
   VtCursor c; c.init(vw, p, job.s, zoff);
   const bool any = c.valid(p);
@@ -225,41 +261,34 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
   uint32_t accumulate = 0;
   for (; c.valid(p); c.next(vw, p, zoff)) {
     mbar_wait(bars.full(r.idx), r.phase);
-    if (live) {
-      const uint64_t da0 = dy_tmpl + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy_wg16);
-      uint64_t db_tap = a_tmpl + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy16 + (uint32_t)(zh0 * HALO_W + zw0));
-      int zw = zw0;
+    const uint64_t da0 = dy_tmpl + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy_wg16);
+    const uint64_t db0 = a_tmpl + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy16);
 #pragma unroll
-      for (int g = 0; g < GMAX; ++g) wgmma_fence_operands(acc[g]);
-      wgmma_fence();
+    for (int g = 0; g < NTAPS; ++g) wgmma_fence_operands(acc[g]);
+    wgmma_fence();
 #pragma unroll
-      for (int g = 0; g < GMAX; ++g) {
-        if (g < ntaps) {
+    for (int g = 0; g < NTAPS; ++g) {
+      uint64_t db = db0 + (uint64_t)tap_off[g];
+      // opaque per stage: otherwise ptxas hoists all NTAPS x 8 loop-invariant B offsets into registers and spills
+      asm volatile("" : "+l"(db));
 #pragma unroll
-          for (int j = 0; j < (TH * TW) / 16; ++j)
-            Wgmma<NTC, 1, 1>::mma(acc[g], da0 + (uint64_t)((uint32_t)j * dy_kstep), db_tap + (uint64_t)((uint32_t)j * a_kstep),
-                                  accumulate | (uint32_t)(j > 0));
-          // next in-plane tap: one voxel to the right, or wrap to the next halo row
-          if (++zw == kw) { zw = 0; db_tap += (uint64_t)(uint32_t)(HALO_W - (kw - 1)); } else db_tap += 1;
-        }
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                             // the group before this one has retired: its stage is free
-#pragma unroll
-      for (int g = 0; g < GMAX; ++g) wgmma_fence_operands(acc[g]);
+      for (int j = 0; j < (TH * TW) / 16; ++j)
+        Wgmma<NTC, 1, 1>::mma(acc[g], da0 + (uint64_t)((uint32_t)j * dy_kstep), db + (uint64_t)((uint32_t)j * a_kstep),
+                              accumulate | (uint32_t)(j > 0));
     }
+    wgmma_commit();
+    wgmma_wait<1>();                               // the group before this one has retired: its stage is free
+#pragma unroll
+    for (int g = 0; g < NTAPS; ++g) wgmma_fence_operands(acc[g]);
     if (pend >= 0 && tid == 0) mbar_arrive(bars.empty(pend));
     pend = r.idx;
     accumulate = 1;
     r.advance();
   }
-  if (live) {
-    wgmma_wait<0>();
+  wgmma_wait<0>();
 #pragma unroll
-    for (int g = 0; g < GMAX; ++g) wgmma_fence_operands(acc[g]);
-  }
+  for (int g = 0; g < NTAPS; ++g) wgmma_fence_operands(acc[g]);
   if (pend >= 0 && tid == 0) mbar_arrive(bars.empty(pend));
-  if (!live) return;
   // S == 1: this CTA is the only contributor of its dW elements, one add each.  S > 1: the partial tile goes to its own
   // slice of the split-K buffer (zeros when the CTA owned no voxel tile) and add_slices sums the slices in order,
   // so dW does not depend on which CTA finishes first.
@@ -273,8 +302,7 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
     const int64_t off = ((int64_t)(co0 + row) * p.Cin + ci0) * taps + tap_base;
     float* drow = p.S > 1 ? p.part + (int64_t)job.s * nw + off : p.dw + off;
 #pragma unroll
-    for (int g = 0; g < GMAX; ++g) {
-      if (g >= ntaps) break;
+    for (int g = 0; g < NTAPS; ++g) {
 #pragma unroll
       for (int j = 0; j < NTC / 8; ++j) {
         const int col = 8 * j + 2 * (lane & 3);
@@ -290,8 +318,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 wgrad_tc_kernel(const __grid_constant__ WgParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  const Job job = decode_job(p, blockIdx.x);
-  const int ci0 = job.ci_tile * p.NTC;
+  const int ci0 = decode_job(p, blockIdx.x).ci_tile * p.NTC;
 
   const Bars bars{smem_u32(smem + p.smem_bar_off), p};
   float2* s_norm = reinterpret_cast<float2*>(smem + p.smem_norm_off);     // [B][NTC] {mean, rstd} of this job's channels
@@ -313,13 +340,27 @@ wgrad_tc_kernel(const __grid_constant__ WgParams p) {
 
   if (warp >= kLoadWarp0) {
     // =========================== LOADERS ===========================
+    setmaxnreg_dec<kRegsLoad>();
+    // each role decodes the job after its setmaxnreg: a value live across the register split is spilled
+    const Job job = decode_job(p, blockIdx.x);
     if (p.prefetch >= 3) wg_loader<3>(p, job, smem, s_norm, bars);
     else if (p.prefetch == 2) wg_loader<2>(p, job, smem, s_norm, bars);
     else wg_loader<1>(p, job, smem, s_norm, bars);
   } else {
     // =========================== MMA + EPILOGUE ===========================
+    setmaxnreg_inc<kRegsConsumer>();
+    const Job job = decode_job(p, blockIdx.x);
     const int wg = warp >> 2, tid = threadIdx.x & 127;
-    dispatch_n(p.NTC, [&](auto ntc) { consumer_role<decltype(ntc)::value>(p, job, wg, tid, smem, bars); });
+    // warpgroup-uniform, and uniform over the CTA's one job: whether this half of the M tile holds real channels,
+    // and how many taps the job's group has
+    if (wg * 64 >= min(MT, p.Cout - job.co_tile * MT)) {
+      idle_consumer_role(p, job, tid, bars);
+    } else {
+      dispatch_n(p.NTC, [&](auto ntc) {
+        constexpr int NTC = decltype(ntc)::value;
+        dispatch_taps<1, max_taps(NTC)>(job.ntaps, [&](auto nt) { consumer_role<NTC, decltype(nt)::value>(p, job, wg, tid, smem, bars); });
+      });
+    }
   }
 }
 
