@@ -11,19 +11,26 @@
 //     wgmma as MN-major no-swizzle matrices (core matrix = 8 voxels x 8 channels, 128 B):
 //     A = dy tile (16x8 voxels), B = halo tile of `a` ((16+kh-1)x(8+kw-1) voxels); a tap is a shifted
 //     B descriptor, exactly like the forward kernel.
-//   * `a` is never materialised by a separate pass: the loader warps stage RAW x with cp.async (up to three stages in
-//     flight) and apply InstanceNorm-normalise + ReLU in place in shared memory once a stage has landed (zero-filled
-//     padding voxels stay zero), exactly like conv_tc.cu's forward loader.
+//   * both operands arrive by tensor TMA: per stage one elected thread issues one box for the dy tile and one for the
+//     x halo tile (tmap.h; out-of-volume voxels are zero-filled by the TMA unit) onto the stage's LAND barrier, as soon
+//     as the consumers hand the slot back, so every free slot of the ring is in flight.
+//   * `a` is never materialised by a separate pass: when x needs InstanceNorm-normalise + activation, the other loader
+//     warps apply it in place in shared memory once a stage has landed (zero-filled padding voxels stay zero, as in
+//     conv_tc.cu's forward loader) and publish FULL; raw x is consumed straight off LAND.
 //   * only the REAL output channels of the M tile are staged (Cout = 32 stages 4 of the 8 planes a warpgroup reads); the
 //     rows computed from whatever follows are never read back.
+//   * the ring holds as many stages as fit (up to 6).  Where fewer than 4 whole 16x8 tiles fit (Cout 128 with a Cin
+//     tile of 80 or more), each tile is staged as two 8-row halves and a stage carries K steps 0-3 or 4-7 of the tile:
+//     the same MMAs in the same order, so dW is the same bit for bit either way.
 //   * split-K over voxel tiles fills the machine: grid = jobs x S.  With S > 1 every CTA stores its partial D tiles
 //     into its own slice of a caller-provided buffer and a second kernel adds the S slices into dW in split order, so
 //     dW is the same bit for bit on every run.
 // Warp roles (512 threads, 1 CTA/SM): warps 0-7 = two MMA warpgroups (output channels 64g .. 64g+63 of the M tile)
-// that also run the epilogue, warps 8-15 loaders.
+// that also run the epilogue, warp 8 = TMA producer (one thread), warps 9-15 = in-place transform.
 #include "common.cuh"
 #include "conv_args.h"
 #include "tc_common.cuh"
+#include "tmap.h"
 #include "wgmma.cuh"
 #include <string.h>
 
@@ -33,35 +40,49 @@ using namespace tc;
 
 constexpr int TH = 16, TW = 8;
 constexpr int kConsumerWGs = 2;
-constexpr int kLoadWarp0 = 8;
-constexpr int kLoadThreads = 256;           // all loader warps cooperate on every stage
+constexpr int kLoadWarp0 = 8;               // TMA producer warp; the transform warps follow it
+constexpr int kXformThreads = 7 * 32;       // warps 9-15 transform every stage together
+constexpr int kMaxStages = 6;
 constexpr int kThreads = 16 * 32;   // 512
 constexpr int MT = 128;                    // output-channel tile (GEMM M)
 constexpr int kMaxCols = 192;              // accumulator columns per job (taps x Cin tile): 96 fp32 registers per thread
 // Registers per thread after the role dispatch, inside the CTA's pool of 512 x 128: the consumer warpgroups hold up to
-// 96 accumulators plus descriptors and epilogue addresses, the loaders' cp.async + transform loop needs far fewer.
+// 96 accumulators plus descriptors and epilogue addresses, the loaders' TMA issue and transform loops need far fewer.
 constexpr int kRegsLaunch = 128, kRegsConsumer = 152, kRegsLoad = 104;
 static_assert(2 * 128 * kRegsConsumer + 2 * 128 * kRegsLoad <= kThreads * kRegsLaunch, "register split exceeds the CTA pool");
 
 struct WgParams {
-  const __half* x; int x_ld, x_coff;       // raw input; normalised + activated on the fly when x_stats / act
-  const double* x_stats; float eps; int act;
-  const __half* dy; int dy_ld, dy_coff;
+  alignas(64) CUtensorMap tm_dy;           // dy as {8 ch, w, h, plane, b*D+d}, box {8, TW, TS, min(Cout, MT)/8}
+  alignas(64) CUtensorMap tm_x;            // x likewise, box {8, HALO_W, HALO_H, NTC/8}
+  const double* x_stats; float eps; int act;   // x is normalised + activated in shared memory when x_stats / act
   float* dw;
   float* part;                             // S > 1: split-K partials [S][Cout][Cin][taps], summed in split order
   int B, D, H, W, Cin, Cout, kd, kh, kw;
   int NTC, ci_tiles, co_tiles, ngroups, gbase, grem, S;
-  int HALO_H, HALO_W, nvox_h, a_plane, dy_plane, a_bytes, dy_bytes, stage_bytes, NS, prefetch;
+  int TS, halves;                          // voxel rows per stage: TH (whole tiles) or TH/2 (two stages per tile)
+  int HALO_H, HALO_W, nvox_h, a_plane, dy_plane, a_bytes, dy_bytes, stage_bytes, NS;
   int tiles_h, tiles_w, nvt;
   int smem_bar_off, smem_norm_off;
 };
 
-// barrier block layout (uint64 each): full[NS] (stage staged and transformed) empty[NS] (stage read by both consumers)
+// barrier block layout (uint64 each): full[NS] (stage transformed) empty[NS] (stage read by both consumers)
+// land[NS] (both TMA boxes of the stage have landed)
 struct Bars {
   uint32_t bar0; const WgParams& p;
   __device__ __forceinline__ uint32_t full(int i) const { return bar0 + 8u * (uint32_t)i; }
   __device__ __forceinline__ uint32_t empty(int i) const { return bar0 + 8u * (uint32_t)(p.NS + i); }
+  __device__ __forceinline__ uint32_t land(int i) const { return bar0 + 8u * (uint32_t)(2 * p.NS + i); }
+  // what the consumers wait on: the transformed stage, or the raw stage straight off the TMA
+  __device__ __forceinline__ uint32_t ready(int i) const { return (p.x_stats || p.act) ? full(i) : land(i); }
 };
+
+// blockIdx.x read afresh: a job decoded again after the register split, or after the MMA loop, is not merged with an
+// earlier decode (whose fields would otherwise stay live, and spill, across it)
+__device__ __forceinline__ int cta_id() {
+  int v;
+  asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(v));
+  return v;
+}
 
 struct Job { int co_tile, ci_tile, zd, grp, tap0, ntaps, s; };
 __device__ __forceinline__ Job decode_job(const WgParams& p, int bid) {
@@ -86,8 +107,9 @@ struct VtWalk {
     s0 = x % r0; x /= r0; s1 = x % r1; x /= r1; s2 = x % r2; s3 = x / r2;
   }
 };
+// A cursor visits the stages of the CTA's tiles in order: every half of a tile (p.halves of them) before the next tile.
 struct VtCursor {
-  int vt, wi, hi, d, b, din;
+  int vt, wi, hi, d, b, din, half;
   __device__ __forceinline__ void step(const VtWalk& k, const WgParams& p) {
     vt += p.S;
     int c;
@@ -100,104 +122,84 @@ struct VtCursor {
     while (vt < p.nvt) { din = d + zoff; if ((unsigned)din < (unsigned)p.D) return; step(k, p); }
   }
   __device__ __forceinline__ void init(const VtWalk& k, const WgParams& p, int s, int zoff) {
-    vt = s;
+    vt = s; half = 0;
     int t = s;
     wi = t % k.r0; t /= k.r0; hi = t % k.r1; t /= k.r1; d = t % k.r2; b = t / k.r2;
     seek(k, p, zoff);
   }
   __device__ __forceinline__ bool valid(const WgParams& p) const { return vt < p.nvt; }
-  __device__ __forceinline__ void next(const VtWalk& k, const WgParams& p, int zoff) { step(k, p); seek(k, p, zoff); }
-  __device__ __forceinline__ int h0() const { return hi * TH; }
+  __device__ __forceinline__ void next(const VtWalk& k, const WgParams& p, int zoff) {
+    if (++half < p.halves) return;
+    half = 0; step(k, p); seek(k, p, zoff);
+  }
+  __device__ __forceinline__ int h0(const WgParams& p) const { return hi * TH + half * p.TS; }     // first row of the stage
   __device__ __forceinline__ int w0() const { return wi * TW; }
 };
 
-template <int P>
-__device__ __forceinline__ void wg_loader(const WgParams& p, const Job& job, uint8_t* smem, const float2* s_norm, const Bars& bars) {
-  const int lt = threadIdx.x - kLoadWarp0 * 32;
+// ---- TMA producer (one thread): per stage, once both consumers have handed the slot back, one box of dy
+// {8 ch, TW, TS, Cout planes} and one box of the x halo {8 ch, HALO_W, HALO_H, NTC/8 planes}, both completing on LAND.
+// Each box lands as [plane][voxel][8 ch] with dense planes; out-of-volume voxels and output channels past Cout are
+// zero-filled and counted in the transaction bytes like any other.
+__device__ __forceinline__ void tma_producer(const WgParams& p, const Job& job, uint8_t* smem, const Bars& bars) {
   const int ph = p.kh / 2, pw = p.kw / 2, zoff = job.zd - p.kd / 2;
-  const int co0 = job.co_tile * MT;
-  const int co_real = min(MT, p.Cout - co0);
-  const int ci0 = job.ci_tile * p.NTC;
-  // dy tile: thread owns plane (lt % cpv) and walks voxels v0, v0+vstep, ...
-  const int cpv_d = co_real / 8;
-  const int vstep_d = kLoadThreads / cpv_d;
-  const bool act_d = lt < vstep_d * cpv_d;
-  const int c8_d = lt % cpv_d, v0_d = lt / cpv_d;
-  const int cpv_a = p.NTC / 8;
-  const int vstep_a = kLoadThreads / cpv_a;
-  const bool act_a = lt < vstep_a * cpv_a;
-  const int c8_a = lt % cpv_a, v0_a = lt / cpv_a;
-  const int sh_a = vstep_a / p.HALO_W, sw_a = vstep_a % p.HALO_W;
-  const int hh0 = v0_a / p.HALO_W, ww0 = v0_a % p.HALO_W;
-  const bool xform = (p.x_stats != nullptr) || (p.act != 0);
+  const int co_p0 = job.co_tile * (MT / 8), ci_p0 = job.ci_tile * (p.NTC / 8);
+  const uint32_t stage_tx = (uint32_t)(p.dy_bytes + (p.NTC / 8) * p.a_plane);
+  VtWalk vw; vw.init(p);
+  VtCursor c; c.init(vw, p, job.s, zoff);
+  Ring r; r.init(p.NS);
+  for (; c.valid(p); c.next(vw, p, zoff)) {
+    mbar_wait(bars.empty(r.idx), r.phase ^ 1);
+    const uint32_t sdy = smem_u32(smem + r.idx * p.stage_bytes);
+    mbar_arrive_expect_tx(bars.land(r.idx), stage_tx);
+    tma_load_5d(sdy, &p.tm_dy, bars.land(r.idx), 0, c.w0(), c.h0(p), co_p0, c.b * p.D + c.d);
+    tma_load_5d(sdy + (uint32_t)p.dy_bytes, &p.tm_x, bars.land(r.idx), 0, c.w0() - pw, c.h0(p) - ph, ci_p0, c.b * p.D + c.din);
+    r.advance();
+  }
+}
+
+// ---- in-place InstanceNorm-normalise + activation of each landed x halo tile (only when x needs it).  Thread owns
+// plane (xt % cpv) and the halo voxels v0, v0 + vstep, ... of it; zero-filled padding voxels stay zero.
+__device__ __forceinline__ void transform_role(const WgParams& p, const Job& job, uint8_t* smem, const float2* s_norm, const Bars& bars) {
+  const int xt = threadIdx.x - (kLoadWarp0 + 1) * 32;
+  const int ph = p.kh / 2, pw = p.kw / 2, zoff = job.zd - p.kd / 2;
+  const int cpv = p.NTC / 8;
+  const int vstep = kXformThreads / cpv;
+  const bool active = xt < vstep * cpv;
+  const int c8 = xt % cpv, v0 = xt / cpv;
+  const int sh = vstep / p.HALO_W, sw = vstep % p.HALO_W;
+  const int hh0 = v0 / p.HALO_W, ww0 = v0 % p.HALO_W;
   const bool relu = p.act == B200SEG_ACT_RELU;
   const float slope = act_slope(p.act);
   VtWalk vw; vw.init(p);
-  VtCursor ci, cd;
-  ci.init(vw, p, job.s, zoff); cd.init(vw, p, job.s, zoff);
-  Ring ri, rd; ri.init(p.NS); rd.init(p.NS);
-
-  auto issue = [&]() {
-    mbar_wait(bars.empty(ri.idx), ri.phase ^ 1);
-    const uint32_t sdy = smem_u32(smem + ri.idx * p.stage_bytes);
-    const uint32_t sa = sdy + (uint32_t)p.dy_bytes;
-    if (act_d) {
-      const __half* src = p.dy + ((int64_t)(ci.b * p.D + ci.d) * p.H * p.W) * p.dy_ld + p.dy_coff + co0 + c8_d * 8;
-      const uint32_t dst = sdy + (uint32_t)(c8_d * p.dy_plane);
-#pragma unroll 4
-      for (int v = v0_d; v < TH * TW; v += vstep_d) {
-        const int h = ci.h0() + (v >> 3), w = ci.w0() + (v & 7);
-        const bool ok = h < p.H && w < p.W;
-        cp_async16(dst + (uint32_t)v * 16u, ok ? (const void*)(src + ((int64_t)h * p.W + w) * p.dy_ld) : (const void*)p.dy, ok ? 16u : 0u);
-      }
-    }
-    if (act_a) {
-      const __half* src = p.x + ((int64_t)(ci.b * p.D + ci.din) * p.H * p.W) * p.x_ld + p.x_coff + ci0 + c8_a * 8;
-      const uint32_t dst = sa + (uint32_t)(c8_a * p.a_plane);
-      int hh = hh0, ww = ww0;
-#pragma unroll 4
-      for (int v = v0_a; v < p.nvox_h; v += vstep_a) {
-        const int h = ci.h0() - ph + hh, w = ci.w0() - pw + ww;
-        const bool ok = (unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W;
-        cp_async16(dst + (uint32_t)v * 16u, ok ? (const void*)(src + ((int64_t)h * p.W + w) * p.x_ld) : (const void*)p.x, ok ? 16u : 0u);
-        hh += sh_a; ww += sw_a;
-        if (ww >= p.HALO_W) { ww -= p.HALO_W; ++hh; }
-      }
-    }
-    ri.advance(); ci.next(vw, p, zoff);
-  };
-
-#pragma unroll
-  for (int i = 0; i < P; ++i) { if (ci.valid(p)) issue(); cp_async_commit(); }
-  while (cd.valid(p)) {
-    cp_async_wait<P - 1>();
-    if (xform && act_a) {
-      uint8_t* sp = smem + rd.idx * p.stage_bytes + p.dy_bytes + c8_a * p.a_plane;
+  VtCursor c; c.init(vw, p, job.s, zoff);
+  Ring r; r.init(p.NS);
+  for (; c.valid(p); c.next(vw, p, zoff)) {
+    mbar_wait(bars.land(r.idx), r.phase);
+    if (active) {
+      uint8_t* sp = smem + r.idx * p.stage_bytes + p.dy_bytes + c8 * p.a_plane;
       float sc[8], sf[8];                          // x*sc + sf == (x - mean) * rstd
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const float2 mr = s_norm[cd.b * p.NTC + c8_a * 8 + j];
+        const float2 mr = s_norm[c.b * p.NTC + c8 * 8 + j];
         sc[j] = mr.y; sf[j] = -mr.x * mr.y;
       }
+      const int hb = c.h0(p) - ph, wb = c.w0() - pw;
       int hh = hh0, ww = ww0;
 #pragma unroll 2
-      for (int v = v0_a; v < p.nvox_h; v += vstep_a) {
-        const int h = cd.h0() - ph + hh, w = cd.w0() - pw + ww;
+      for (int v = v0; v < p.nvox_h; v += vstep) {
+        const int h = hb + hh, w = wb + ww;
         if ((unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W) {      // padding voxels stay zero
           uint4* chunk = reinterpret_cast<uint4*>(sp + v * 16);
           *chunk = relu ? norm_act8<true>(*chunk, sc, sf, slope) : norm_act8<false>(*chunk, sc, sf, slope);
         }
-        hh += sh_a; ww += sw_a;
+        hh += sh; ww += sw;
         if (ww >= p.HALO_W) { ww -= p.HALO_W; ++hh; }
       }
     }
-    fence_proxy_async();
-    mbar_arrive(bars.full(rd.idx));
-    rd.advance(); cd.next(vw, p, zoff);
-    if (ci.valid(p)) issue();
-    cp_async_commit();
+    fence_proxy_async();                           // generic-proxy writes -> visible to the tensor core (async proxy)
+    mbar_arrive(bars.full(r.idx));
+    r.advance();
   }
-  cp_async_wait<0>();
 }
 
 // most taps one job's group can have at Cin tile NTC (fill_params: G = min(kMaxCols / NTC, kh * kw), kh, kw <= 3)
@@ -220,21 +222,22 @@ __device__ __forceinline__ void idle_consumer_role(const WgParams& p, const Job&
   VtCursor c; c.init(vw, p, job.s, zoff);
   Ring r; r.init(p.NS);
   for (; c.valid(p); c.next(vw, p, zoff)) {
-    mbar_wait(bars.full(r.idx), r.phase);
+    mbar_wait(bars.ready(r.idx), r.phase);
     if (tid == 0) mbar_arrive(bars.empty(r.idx));
     r.advance();
   }
 }
 
-// ---- MMA warpgroup g: output channels co0 + 64g .. +63 of the M tile, the NTAPS taps of the job's group.  Per voxel
-// tile one wgmma group (NTAPS x 8 instructions m64 x NTC x 16) is committed; the stage the group before it read is then
-// handed back.  After the last tile the accumulators are added into dW (thread: rows 16w + l/4 (+8), column pairs
-// 8j + 2(l%4)).  NTAPS is a template argument and the group has no branch: a run-time tap count made ptxas retire every
-// group before the next one could issue (C7517), which undid the one-group-in-flight pipelining.
-template <int NTC, int NTAPS>
+// ---- MMA warpgroup g: output channels co0 + 64g .. +63 of the M tile, the NTAPS taps of the job's group.  Per stage
+// one wgmma group (NTAPS x KS instructions m64 x NTC x 16; KS = 8 for a whole 16x8 tile, 4 for a half) is committed;
+// the stage the group before it read is then handed back.  Each accumulator sees K steps 0-7 of every tile in order,
+// whether a tile arrives in one stage or two.  After the last tile the accumulators are added into dW (thread: rows
+// 16w + l/4 (+8), column pairs 8j + 2(l%4)).  NTAPS and KS are template arguments and the group has no branch: a
+// run-time tap count made ptxas retire every group before the next one could issue (C7517), which undid the
+// one-group-in-flight pipelining.
+template <int NTC, int NTAPS, int KS>
 __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job, int wg, int tid, uint8_t* smem, const Bars& bars) {
   const int zoff = job.zd - p.kd / 2;
-  const int co0 = job.co_tile * MT, co_real = min(MT, p.Cout - co0), ci0 = job.ci_tile * NTC;
   // dy^T as the A operand: MN-major (lbo = next 8 voxels, sbo = next channel plane); x halo tile as the B operand:
   // MN-major (lbo = next halo row of voxels, sbo = next channel plane), a tap = start shifted by whole voxel slots
   const uint64_t dy_tmpl = make_desc(0, 128u, (uint32_t)p.dy_plane);
@@ -260,7 +263,7 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
   int pend = -1;
   uint32_t accumulate = 0;
   for (; c.valid(p); c.next(vw, p, zoff)) {
-    mbar_wait(bars.full(r.idx), r.phase);
+    mbar_wait(bars.ready(r.idx), r.phase);
     const uint64_t da0 = dy_tmpl + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy_wg16);
     const uint64_t db0 = a_tmpl + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy16);
 #pragma unroll
@@ -272,7 +275,7 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
       // opaque per stage: otherwise ptxas hoists all NTAPS x 8 loop-invariant B offsets into registers and spills
       asm volatile("" : "+l"(db));
 #pragma unroll
-      for (int j = 0; j < (TH * TW) / 16; ++j)
+      for (int j = 0; j < KS; ++j)
         Wgmma<NTC, 1, 1>::mma(acc[g], da0 + (uint64_t)((uint32_t)j * dy_kstep), db + (uint64_t)((uint32_t)j * a_kstep),
                               accumulate | (uint32_t)(j > 0));
     }
@@ -292,15 +295,17 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
   // S == 1: this CTA is the only contributor of its dW elements, one add each.  S > 1: the partial tile goes to its own
   // slice of the split-K buffer (zeros when the CTA owned no voxel tile) and add_slices sums the slices in order,
   // so dW does not depend on which CTA finishes first.
+  const Job e = decode_job(p, cta_id());
+  const int co0 = e.co_tile * MT, co_real = min(MT, p.Cout - co0), ci0 = e.ci_tile * NTC;
   const int warp = tid >> 5, lane = tid & 31;
-  const int taps = p.kd * p.kh * p.kw, tap_base = job.zd * p.kh * p.kw + job.tap0;
+  const int taps = p.kd * p.kh * p.kw, tap_base = e.zd * p.kh * p.kw + e.tap0;
   const int64_t nw = (int64_t)p.Cout * p.Cin * taps;
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const int row = wg * 64 + 16 * warp + (lane >> 2) + 8 * i;
     if (row >= co_real) continue;
     const int64_t off = ((int64_t)(co0 + row) * p.Cin + ci0) * taps + tap_base;
-    float* drow = p.S > 1 ? p.part + (int64_t)job.s * nw + off : p.dw + off;
+    float* drow = p.S > 1 ? p.part + (int64_t)e.s * nw + off : p.dw + off;
 #pragma unroll
     for (int g = 0; g < NTAPS; ++g) {
 #pragma unroll
@@ -324,7 +329,9 @@ wgrad_tc_kernel(const __grid_constant__ WgParams p) {
   float2* s_norm = reinterpret_cast<float2*>(smem + p.smem_norm_off);     // [B][NTC] {mean, rstd} of this job's channels
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < p.NS; ++i) { mbar_init(bars.full(i), kLoadThreads); mbar_init(bars.empty(i), kConsumerWGs); }
+    for (int i = 0; i < p.NS; ++i) {
+      mbar_init(bars.full(i), kXformThreads); mbar_init(bars.empty(i), kConsumerWGs); mbar_init(bars.land(i), 1);
+    }
     fence_barrier_init();
   }
   {
@@ -342,14 +349,16 @@ wgrad_tc_kernel(const __grid_constant__ WgParams p) {
     // =========================== LOADERS ===========================
     setmaxnreg_dec<kRegsLoad>();
     // each role decodes the job after its setmaxnreg: a value live across the register split is spilled
-    const Job job = decode_job(p, blockIdx.x);
-    if (p.prefetch >= 3) wg_loader<3>(p, job, smem, s_norm, bars);
-    else if (p.prefetch == 2) wg_loader<2>(p, job, smem, s_norm, bars);
-    else wg_loader<1>(p, job, smem, s_norm, bars);
+    const Job job = decode_job(p, cta_id());
+    if (warp == kLoadWarp0) {
+      if ((threadIdx.x & 31) == 0) tma_producer(p, job, smem, bars);
+    } else if (p.x_stats || p.act) {
+      transform_role(p, job, smem, s_norm, bars);
+    }
   } else {
     // =========================== MMA + EPILOGUE ===========================
     setmaxnreg_inc<kRegsConsumer>();
-    const Job job = decode_job(p, blockIdx.x);
+    const Job job = decode_job(p, cta_id());
     const int wg = warp >> 2, tid = threadIdx.x & 127;
     // warpgroup-uniform, and uniform over the CTA's one job: whether this half of the M tile holds real channels,
     // and how many taps the job's group has
@@ -358,7 +367,11 @@ wgrad_tc_kernel(const __grid_constant__ WgParams p) {
     } else {
       dispatch_n(p.NTC, [&](auto ntc) {
         constexpr int NTC = decltype(ntc)::value;
-        dispatch_taps<1, max_taps(NTC)>(job.ntaps, [&](auto nt) { consumer_role<NTC, decltype(nt)::value>(p, job, wg, tid, smem, bars); });
+        dispatch_taps<1, max_taps(NTC)>(job.ntaps, [&](auto nt) {
+          constexpr int NTAPS = decltype(nt)::value;
+          if (p.halves == 2) consumer_role<NTC, NTAPS, TH / 4>(p, job, wg, tid, smem, bars);
+          else consumer_role<NTC, NTAPS, TH / 2>(p, job, wg, tid, smem, bars);
+        });
       });
     }
   }
@@ -387,21 +400,30 @@ bool fill_params(const WgradArgs& a, WgParams& p) {
   int G = kMaxCols / p.NTC; if (G > taps_hw) G = taps_hw;
   p.ngroups = (taps_hw + G - 1) / G;
   p.gbase = taps_hw / p.ngroups; p.grem = taps_hw % p.ngroups;
-  p.HALO_H = TH + a.kh - 1; p.HALO_W = TW + a.kw - 1; p.nvox_h = p.HALO_H * p.HALO_W;
-  int slots = p.nvox_h; if ((slots & 1) == 0) ++slots;
-  p.a_plane = slots * 16;
-  p.dy_plane = (TH * TW + 1) * 16;
-  p.a_bytes = (p.NTC / 8) * p.a_plane; p.a_bytes = (p.a_bytes + 127) / 128 * 128;
-  // only the real output-channel planes of the widest M tile are staged; the descriptors' 8-plane footprint beyond
-  // them falls on the `a` tile / the next stage / the tail slack (allocated below), whose values feed rows never read
+  p.HALO_W = TW + a.kw - 1;
+  // only the real output-channel planes of the widest M tile are staged; a consumer warpgroup's A descriptor spans 8
+  // whole planes, so with Cout not a multiple of 64 the last live warpgroup reads past them into the `a` tile, the
+  // next stage or, from the last slot, the tail (rows computed from those values are never read back)
   const int co_max = a.Cout < MT ? a.Cout : MT;
-  p.dy_bytes = (co_max / 8) * p.dy_plane; p.dy_bytes = (p.dy_bytes + 127) / 128 * 128;
-  p.stage_bytes = p.a_bytes + p.dy_bytes;
   const int norm_bytes = a.B * p.NTC * 8;
-  const int budget = 227 * 1024 - 2048 - 16 * p.dy_plane - norm_bytes;
-  p.NS = budget / p.stage_bytes; if (p.NS > 6) p.NS = 6;
+  int tail = 0;
+  auto size_ring = [&](int ts) {
+    p.TS = ts; p.halves = TH / ts;
+    p.HALO_H = ts + a.kh - 1; p.nvox_h = p.HALO_H * p.HALO_W;
+    p.a_plane = p.nvox_h * 16;                 // TMA boxes land with dense planes
+    p.dy_plane = ts * TW * 16;
+    p.a_bytes = (p.NTC / 8) * p.a_plane; p.a_bytes = (p.a_bytes + 127) / 128 * 128;
+    p.dy_bytes = (co_max / 8) * p.dy_plane;    // a multiple of 1024: the `a` box starts 128-byte aligned
+    p.stage_bytes = p.a_bytes + p.dy_bytes;
+    const int span = (co_max + 63) / 64 * 8 * p.dy_plane;
+    tail = span > p.stage_bytes ? span - p.stage_bytes : 0;
+    p.NS = (227 * 1024 - 2048 - tail - norm_bytes) / p.stage_bytes;
+    if (p.NS > kMaxStages) p.NS = kMaxStages;
+  };
+  // whole 16x8 tiles, or two 8-row halves per tile where fewer than 4 whole tiles fit
+  size_ring(TH);
+  if (p.NS < 4) size_ring(TH / 2);
   if (p.NS < 2) return false;
-  p.prefetch = p.NS - 1 < 3 ? p.NS - 1 : 3;
   p.tiles_h = (a.H + TH - 1) / TH; p.tiles_w = (a.W + TW - 1) / TW;
   const int64_t nvt = (int64_t)a.B * a.D * p.tiles_h * p.tiles_w;
   if (nvt > 0x7fffffff) return false;
@@ -410,9 +432,9 @@ bool fill_params(const WgradArgs& a, WgParams& p) {
   int S = (int)(B200SEG_NUM_SMS / jobs); if (S < 1) S = 1;
   if (S > p.nvt) S = p.nvt;
   p.S = S;
-  int off = p.NS * p.stage_bytes + 16 * p.dy_plane;       // + slack for the 16-plane descriptor footprint
+  int off = p.NS * p.stage_bytes + tail;
   off = (off + 15) / 16 * 16;
-  p.smem_bar_off = off; off += 2 * p.NS * 8;
+  p.smem_bar_off = off; off += 3 * p.NS * 8;
   off = (off + 15) / 16 * 16;
   p.smem_norm_off = off;
   return true;
@@ -444,9 +466,12 @@ int conv3d_wgrad_tc(const WgradArgs& a, int dtype, void* workspace, size_t ws_by
   if (need && (!workspace || ws_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 15))) return B200SEG_EINVAL;
   WgParams p;
   fill_params(a, p);
-  p.x = reinterpret_cast<const __half*>(a.x); p.x_ld = a.x_ld; p.x_coff = a.x_coff;
+  // the alignment conditions of conv3d_wgrad_tc_supported are the ones TMA needs; only a missing driver entry point
+  // can make this fail
+  if (!b200seg_make_act_tmap(&p.tm_dy, a.dy, a.dy_ld, a.dy_coff, a.Cout, a.B * a.D, a.H, a.W, TW, p.TS, (a.Cout < MT ? a.Cout : MT) / 8) ||
+      !b200seg_make_act_tmap(&p.tm_x, a.x, a.x_ld, a.x_coff, a.Cin, a.B * a.D, a.H, a.W, p.HALO_W, p.HALO_H, p.NTC / 8))
+    return B200SEG_ECUDA;
   p.x_stats = a.x_stats; p.eps = a.eps; p.act = a.act;
-  p.dy = reinterpret_cast<const __half*>(a.dy); p.dy_ld = a.dy_ld; p.dy_coff = a.dy_coff;
   p.dw = a.dw;
   const int64_t jobs = (int64_t)p.co_tiles * p.ci_tiles * a.kd * p.ngroups;
   const int smem_bytes = p.smem_norm_off + a.B * p.NTC * 8 + 64;
