@@ -7,7 +7,7 @@ from . import augmentation
 from ._lib import B200SegError, EXPORTED_SYMBOLS, LIB_PATH
 from .attention_unet import AttentionUNet
 from .factory import get_model
-from .inference import (calculate_dice, calculate_dice_split, get_inference, inference_sliding_window,
+from .inference import (calculate_dice, calculate_dice_split, calculate_distance, get_inference, inference_sliding_window,
                         inference_whole_image)
 from .losses import CrossEntropyLoss, DiceCELoss, DiceLoss
 from .medformer import MedFormer
@@ -18,4 +18,4 @@ from .unetr import UNETR
 
 __all__ = ["augmentation", "get_model", "UNet", "MedFormer", "SwinUNETR", "UNETR", "UNetPlusPlus", "AttentionUNet", "DiceLoss", "DiceCELoss", "CrossEntropyLoss", "B200SegError",
            "EXPORTED_SYMBOLS", "LIB_PATH", "get_inference", "inference_sliding_window", "inference_whole_image",
-           "calculate_dice", "calculate_dice_split"]
+           "calculate_dice", "calculate_dice_split", "calculate_distance"]

@@ -73,6 +73,9 @@ _PROTOS = {
     "b200seg_softmax_accumulate": [P, I, L, L, L, P, P, I, I, I, I, I, I, I, I, I, I, I, P],
     "b200seg_normalize_argmax": [P, P, P, I, I, L, P],
     "b200seg_dice_metric": [P, I, P, I, L, I, P, P],
+    "b200seg_surface_distance_workspace": [I, I, I, I],
+    "b200seg_surface_distance": [P, I, P, I, I, I, I, I, c_double, c_double, c_double, c_double, P, P, P, P,
+                                 ctypes.c_size_t, P],
     "b200seg_aug_resample": [P, P, I, I, P, P, P, P, P, P, I, P, P, I, P, I, P],
     "b200seg_aug_pointwise": [P, P, I, L, I, P, P, P, P, P, ctypes.c_uint64, P],
     "b200seg_aug_gaussian_blur": [P, P, I, I, I, I, P, I, P, I, P],
@@ -85,7 +88,8 @@ _PROTOS = {
 }
 _RESTYPES = {"b200seg_strerror": c_char_p, "b200seg_last_cuda_error": c_char_p,
              "b200seg_conv3d_wgrad_workspace": ctypes.c_size_t, "b200seg_biattn_workspace": ctypes.c_size_t,
-             "b200seg_mapgen_workspace": ctypes.c_size_t, "b200seg_window_attn_workspace": ctypes.c_size_t}
+             "b200seg_mapgen_workspace": ctypes.c_size_t, "b200seg_window_attn_workspace": ctypes.c_size_t,
+             "b200seg_surface_distance_workspace": ctypes.c_size_t}
 
 EXPORTED_SYMBOLS = tuple(_PROTOS)
 

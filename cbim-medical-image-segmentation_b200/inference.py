@@ -1,15 +1,19 @@
 """Evaluation-side consumers of ``net(x)`` behind the reference's own function names (SURVEY.md §8f.2):
   inference_whole_image / inference_sliding_window / get_inference   inference/inference3d.py:8-92, inference/utils.py:1-40
   calculate_dice / calculate_dice_split                               metric/utils.py:33-82
+  calculate_distance                                                  metric/utils.py:8-28
 Same signatures and return values (probabilities fp32 [B,classes,D,H,W]; (dice, intersection, summ) tensors); the
 window schedule (half-window stride, last window snapped to the border, utils.split_idx) is the reference's.  On the
 device the per-window softmax + accumulate + count is ONE kernel, the final division (and an optional argmax label
-map) another, and the Dice metric is a single pass over the two label maps — the [N,C] one-hot masks never exist."""
+map) another, and the Dice metric is a single pass over the two label maps — the [N,C] one-hot masks never exist.
+The surface distances (ASD, percentile HD) run on the device too (csrc/surface.cu, DESIGN.md §3.10)."""
+import numpy as np
 import torch
 import torch.nn.functional as F
 
 from . import _lib
 from .ops import _dt, _need_cuda, _stream, on_device
+from .surface import surface_area_table
 
 
 def split_idx(half_win, size, i):
@@ -127,3 +131,43 @@ def calculate_dice_split(pred, target, C, block_size=64 * 64 * 64):
     _, inter, summ = calculate_dice(pred, target, C)
     summ = summ - 1e-5
     return 2 * inter / (summ + 1e-5), inter, summ
+
+
+def calculate_distance(label_pred, label_true, spacing, C, percentage=95):
+    """metric/utils.py:8-28: label maps [D,H,W] (CUDA, any integer dtype; uint8 / int64 are read in place), spacing
+    (tensor, ndarray or sequence of 3) -> (ASD_list, HD_list), numpy float64 [C-1]: per class 1..C-1 the mean of the
+    two directed average surface distances and the larger of the two directed `percentage` percentile distances.
+    A class missing from one or both maps gives nan / inf, as the reference (validation_ddp clips them itself)."""
+    if label_pred.dim() != 3 or label_true.dim() != 3:
+        raise ValueError("calculate_distance takes 3-D label maps, got %d-D and %d-D" % (label_pred.dim(), label_true.dim()))
+    if label_pred.shape != label_true.shape:
+        raise ValueError("label maps differ in shape: %s vs %s" % (tuple(label_pred.shape), tuple(label_true.shape)))
+    if C > 256:
+        raise _lib.B200SegError("calculate_distance supports at most 256 classes, got %d" % C)
+    _need_cuda(label_pred)
+    _need_cuda(label_true)
+    if isinstance(spacing, torch.Tensor):
+        spacing = spacing.detach().cpu().double().tolist()
+    spacing = [float(s) for s in np.asarray(spacing, dtype=np.float64).reshape(-1)]
+    table = surface_area_table(spacing)
+    maps = []
+    for t in (label_pred, label_true):
+        if t.dtype not in (torch.uint8, torch.int64):
+            t = t.long()
+        maps.append(t.contiguous())
+    p, t = maps
+    D, H, W = p.shape
+    if C < 2:
+        return np.zeros(0), np.zeros(0)
+    with on_device(p):
+        table_d = torch.from_numpy(table).to(p.device)
+        out = torch.empty(2, C - 1, dtype=torch.float64, device=p.device)
+        ws_bytes = _lib.load().b200seg_surface_distance_workspace(D, H, W, C)
+        if ws_bytes == 0:
+            raise _lib.B200SegError("calculate_distance: unsupported volume %dx%dx%d" % (D, H, W))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=p.device)
+        _lib.call("b200seg_surface_distance", p.data_ptr(), p.element_size(), t.data_ptr(), t.element_size(), D, H, W, C,
+                  spacing[0], spacing[1], spacing[2], float(percentage), table_d.data_ptr(), out[0].data_ptr(),
+                  out[1].data_ptr(), ws.data_ptr(), ws_bytes, _stream())
+        res = out.cpu().numpy()
+    return res[0].copy(), res[1].copy()

@@ -444,6 +444,21 @@ int b200seg_dice_metric(const void* pred, int pred_bytes, const void* target, in
                         int64_t N, int C, unsigned long long* out, void* stream);
 
 /* ---------------------------------------------------------------------------
+ * Validation surface distances: metric/utils.py:8-28 (calculate_distance) with the semantics of
+ * metric/metrics.py:265-720.  For every class c in 1..C-1 of the label maps gt / pred (uint8 or int64,
+ * bytes = 1 / 8, [D][H][W]): asd[c-1] = the mean of the two directed area-weighted average surface distances,
+ * hd[c-1] = the larger of the two directed `percent` percentile distances (fp64, device pointers).  A class
+ * absent from one or both maps gives nan / inf, as the reference.  table: device fp64 [256] surfel area per
+ * neighbour code at spacing (s0, s1, s2) (b200seg.surface.surface_area_table).  Results are bit-identical
+ * from run to run.  The call waits for one small device-to-host copy (the per-class bounding boxes).
+ * workspace: b200seg_surface_distance_workspace() bytes (0: unsupported size, C > 256).
+ * ------------------------------------------------------------------------- */
+size_t b200seg_surface_distance_workspace(int D, int H, int W, int C);
+int b200seg_surface_distance(const void* pred, int pred_bytes, const void* gt, int gt_bytes, int D, int H, int W,
+                             int C, double s0, double s1, double s2, double percent, const double* table,
+                             double* asd, double* hd, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------
  * GPU augmentation (SURVEY.md 8f.3; `aug_device: gpu`, training/augmentation.py, driven per sample by
  * training/dataset/dim3/dataset_kits.py:116-153).  Images are fp32 [C][D][H][W] (the reference's
  * [1,C,D,H,W]); label maps uint8 (bytes = 1) or int64 (bytes = 8).  The small geometry / parameter
