@@ -21,9 +21,14 @@ namespace {
 
 using namespace swin;
 
+// a padding token's q / k / v is the qkv bias as the reference's Linear returns it for a zero input: in the activation
+// type, i.e. rounded to fp16 under autocast (as swin_mma.cu's load_token does)
+template <typename T> __device__ __forceinline__ float pad_value(float b) { return b; }
+template <> __device__ __forceinline__ float pad_value<__half>(float b) { return __half2float(__float2half_rn(b)); }
+
 template <typename T>
 __device__ __forceinline__ void load_vec(const T* p, const float* bias, bool valid, int dh, float* out) {
-  for (int d = 0; d < dh; ++d) out[d] = valid ? Elem<T>::ld(p + d) : (bias ? bias[d] : 0.f);
+  for (int d = 0; d < dh; ++d) out[d] = valid ? Elem<T>::ld(p + d) : (bias ? pad_value<T>(bias[d]) : 0.f);
 }
 
 // shared layout: K[n][dh], V[n][dh] (fp32), table[T] (this head's bias column), rid[n], rc[n]

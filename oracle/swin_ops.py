@@ -8,6 +8,7 @@ SwinUNETR whose behaviour can be pinned here, because it does not live in the ab
   compute_mask                   swin_unetr.py:737-773
   window_attention               WindowAttention.forward     swin_unetr.py:467-490
   swin_block_part1               SwinTransformerBlock.forward_part1  swin_unetr.py:554-606
+  window_attention_core          forward_part1 between the qkv and proj Linears, chunked (the window-attention kernels' operator)
   patch_merging                  PatchMerging.forward (v0.9 ordering, with its duplicated slices)  swin_unetr.py:707-731
 Pinned by oracle/make_golden_swin.py against the unmodified classes (imported with a throw-away stand-in for the
 seven monai symbols the file pulls in) -> tests/golden/swin_*.pt.  The monai-defined blocks (MLPBlock, PatchEmbed,
@@ -111,6 +112,93 @@ def swin_block_part1(x, p, heads, window_size, shift_size, mask_matrix):
     if shifted:
         x = torch.roll(x, shifts=(ss[0], ss[1], ss[2]), dims=(1, 2, 3))
     return x[:, :d, :h, :w, :].contiguous()
+
+
+def _round16(t):
+    """t rounded to fp16 in value, with an identity gradient (autocast rounds the forward value only)."""
+    return t + (t.half().to(t.dtype) - t).detach()
+
+
+def _attention_core(x, table, rel, mask, heads, fp16_rounding):
+    """x [w, n, 3C] partitioned qkv windows -> [w, n, C]: the middle of WindowAttention.forward, swin_unetr.py:467-490.
+    mask [w, n, n] or None."""
+    w, n, c3 = x.shape
+    c = c3 // 3
+    qkv = x.reshape(w, n, 3, heads, c // heads).permute(2, 0, 3, 1, 4)
+    q, k, v = qkv[0] * (c // heads) ** -0.5, qkv[1], qkv[2]
+    if fp16_rounding:
+        q = _round16(q)                                      # autocast: `q * self.scale` is an fp16 tensor
+    attn = q @ k.transpose(-2, -1) + table[rel.reshape(-1)].reshape(n, n, heads).permute(2, 0, 1).unsqueeze(0)
+    if mask is not None:
+        attn = attn + mask.unsqueeze(1)
+    attn = F.softmax(attn, dim=-1)
+    if fp16_rounding:
+        attn = _round16(attn)                                # `attn.to(v.dtype)` before `@ v`
+    return (attn @ v).transpose(1, 2).reshape(w, n, c)
+
+
+class _ChunkedCore(torch.autograd.Function):
+    """_attention_core over chunks of windows; the backward recomputes each chunk, so the [w, heads, n, n] scores of one
+    chunk at a time are all that is ever held (stage 1 of a 128^3 SwinUNETR has 1000 windows of 343 tokens)."""
+
+    @staticmethod
+    def forward(ctx, xw, table, rel, mask, heads, fp16_rounding, chunk):
+        ctx.save_for_backward(xw, table, rel, mask)
+        ctx.meta = (heads, fp16_rounding, chunk)
+        nw = 1 if mask is None else mask.shape[0]
+        outs = []
+        for i in range(0, xw.shape[0], chunk):
+            j = min(i + chunk, xw.shape[0])
+            m = None if mask is None else mask[torch.arange(i, j, device=xw.device) % nw]
+            outs.append(_attention_core(xw[i:j], table, rel, m, heads, fp16_rounding))
+        return torch.cat(outs)
+
+    @staticmethod
+    def backward(ctx, dout):
+        xw, table, rel, mask = ctx.saved_tensors
+        heads, fp16_rounding, chunk = ctx.meta
+        nw = 1 if mask is None else mask.shape[0]
+        dx, dt = torch.empty_like(xw), torch.zeros_like(table)
+        for i in range(0, xw.shape[0], chunk):
+            j = min(i + chunk, xw.shape[0])
+            m = None if mask is None else mask[torch.arange(i, j, device=xw.device) % nw]
+            with torch.enable_grad():
+                x, t = xw[i:j].detach().requires_grad_(True), table.detach().requires_grad_(True)
+                gx, gt = torch.autograd.grad(_attention_core(x, t, rel, m, heads, fp16_rounding), (x, t), dout[i:j])
+            dx[i:j] = gx
+            dt += gt
+        return dx, dt, None, None, None, None, None
+
+
+def window_attention_core(qkv, qkv_bias, table, heads, window, shift, fp16_rounding=False, chunk=64):
+    """qkv [B,D,H,W,3C] -> attention output [B,D,H,W,C]: SwinTransformerBlock.forward_part1 between the qkv and proj
+    Linears (swin_unetr.py:554-606), i.e. the operator of the project's window-attention kernels, differentiable in qkv,
+    qkv_bias ([3C] or None) and table ([T, heads]).
+      * The reference pads after norm1 and before the qkv Linear, so a padding token's q/k/v is the qkv bias.  Written
+        as pad(qkv - b) + b, autograd sends exactly the padding region's gradient to b.
+      * fp16_rounding: round where the reference's autocast rounds: the bias (an fp16 Linear on a zero input returns
+        fp16(b)), q * scale, and the probabilities before `@ v`.  The rounding has an identity gradient.
+      * The window is clamped (and its shift dropped) on axes not larger than it; the relative-position index is the
+        nominal window's, sliced [:n, :n] (swin_unetr.py:474)."""
+    B, D, H, W, C3 = qkv.shape
+    ws, ss = get_window_size((D, H, W), window, shift)
+    b = torch.zeros(C3, dtype=qkv.dtype, device=qkv.device) if qkv_bias is None else qkv_bias.to(qkv.dtype)
+    if fp16_rounding:
+        b = _round16(b)
+    pads = [(ws[i] - s % ws[i]) % ws[i] for i, s in enumerate((D, H, W))]
+    x = F.pad(qkv - b, (0, 0, 0, pads[2], 0, pads[1], 0, pads[0])) + b
+    dp, hp, wp = x.shape[1:4]
+    shifted = any(s > 0 for s in ss)
+    if shifted:
+        x = torch.roll(x, shifts=(-ss[0], -ss[1], -ss[2]), dims=(1, 2, 3))
+    n = ws[0] * ws[1] * ws[2]
+    rel = relative_position_index(window)[:n, :n].to(qkv.device)
+    mask = compute_mask((dp, hp, wp), ws, ss).to(qkv.device, qkv.dtype) if shifted else None
+    out = _ChunkedCore.apply(window_partition(x, ws), table.to(qkv.dtype), rel, mask, heads, fp16_rounding, chunk)
+    x = window_reverse(out, ws, [B, dp, hp, wp])
+    if shifted:
+        x = torch.roll(x, shifts=ss, dims=(1, 2, 3))
+    return x[:, :D, :H, :W, :]
 
 
 def patch_merging(x, norm_w, norm_b, red_w):

@@ -23,6 +23,30 @@ def test_state_dict_contract():
         b200seg.SwinUNETR(c["size"], c["in_ch"], c["classes"], feature_size=20)          # feature_size % 12 (the reference's check)
 
 
+@pytest.mark.parametrize("name", ["swin_block_a", "swin_block_b", "swin_block_c"])
+@pytest.mark.parametrize("chunk", [64, 1])
+def test_window_attention_core_reproduces_block_fixtures(name, chunk):
+    """oracle.swin_ops.window_attention_core, the fp64 statement the GPU window-attention tests compare against, composed
+    as LayerNorm -> qkv Linear -> window_attention_core -> proj reproduces the reference's SwinTransformerBlock
+    .forward_part1 (padding, shift, clamped window) and every one of its gradients, including the bias table and qkv_b."""
+    import torch.nn.functional as F
+    from oracle import swin_ops as so
+    g = load_golden(name)
+    cfg = g["cfg"]
+    p = {k: v.double().clone().requires_grad_(True) for k, v in g["params"].items()}
+    x = g["x"].double().clone().requires_grad_(True)
+    xn = F.layer_norm(x, (x.shape[-1],), p["norm1_w"], p["norm1_b"])
+    qkv = F.linear(xn, p["qkv_w"], p["qkv_b"])
+    att = so.window_attention_core(qkv, p["qkv_b"], p["bias_table"], cfg["heads"], cfg["window"], cfg["shift"], chunk=chunk)
+    y = F.linear(att, p["proj_w"], p["proj_b"])
+    y.backward(g["gy"].double())
+    # the fixtures are the reference's fp32 numbers: 4e-7 is the largest distance measured
+    assert rel_err(y, g["y"]) < 2e-6
+    assert rel_err(x.grad, g["dx"]) < 2e-6
+    errs = {k: rel_err(p[k].grad, g["dparams"][k]) for k in p}
+    assert max(errs.values()) < 2e-6, errs
+
+
 def test_orchestration_matches_oracle(monkeypatch):
     emu_swin.install(monkeypatch)
     size, classes, fs = (64, 32, 32), 3, 12          # deepest level 2x1x1: InstanceNorm needs more than one voxel
