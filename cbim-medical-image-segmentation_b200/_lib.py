@@ -53,7 +53,8 @@ _PROTOS = {
     "b200seg_se_gate_fwd": [P, L, P, P, P, P, P, P, P, I, I, I, P],
     "b200seg_se_gate_bwd": [P, P, P, P, P, P, P, P, P, P, P, I, I, I, P],
     "b200seg_channel_scale_fwd": [P, P, P, I, L, I, I, P],
-    "b200seg_channel_scale_bwd_reduce": [P, P, P, I, L, I, I, P],
+    "b200seg_channel_scale_bwd_workspace": [I, L, I],
+    "b200seg_channel_scale_bwd_reduce": [P, P, P, P, I, L, I, I, P],
     "b200seg_channel_scale_bwd_apply": [P, P, P, P, I, L, I, I, P],
     "b200seg_layernorm_fwd": [P, P, P, P, P, I, I, F, I, P],
     "b200seg_layernorm_bwd": [P, P, P, P, P, P, P, I, I, I, P],
@@ -88,7 +89,8 @@ _PROTOS = {
 }
 _RESTYPES = {"b200seg_strerror": c_char_p, "b200seg_last_cuda_error": c_char_p,
              "b200seg_conv3d_wgrad_workspace": ctypes.c_size_t, "b200seg_biattn_workspace": ctypes.c_size_t,
-             "b200seg_mapgen_workspace": ctypes.c_size_t, "b200seg_window_attn_workspace": ctypes.c_size_t,
+             "b200seg_mapgen_workspace": ctypes.c_size_t,
+             "b200seg_channel_scale_bwd_workspace": ctypes.c_size_t, "b200seg_window_attn_workspace": ctypes.c_size_t,
              "b200seg_surface_distance_workspace": ctypes.c_size_t}
 
 EXPORTED_SYMBOLS = tuple(_PROTOS)
@@ -128,7 +130,7 @@ def check(rc, what):
 
 # kernels launched per entry point (dice fwd = reduce + finalize; its memset is not ours)
 _KERNELS = {"b200seg_dice_ce_fwd": 2, "b200seg_biattn_fwd": 2, "b200seg_window_attn_bwd": 2, "b200seg_attention_bwd": 3, "b200seg_adamw_ema_step": 2, "b200seg_biattn_bwd": 2,
-            "b200seg_mapgen_fwd": 2, "b200seg_attn_gate_fwd": 2, "b200seg_attn_gate_bwd": 2}
+            "b200seg_mapgen_fwd": 2, "b200seg_channel_scale_bwd_reduce": 2, "b200seg_attn_gate_fwd": 2, "b200seg_attn_gate_bwd": 2}
 launch_count = 0
 
 

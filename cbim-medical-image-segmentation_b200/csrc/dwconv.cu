@@ -66,8 +66,8 @@ __global__ void __launch_bounds__(256, 2) dwconv_fwd_kernel(DwArgs a) {
   float* s_w = sm;                         // [taps][C]
   float* s_scale = s_w + taps * C;         // [C]
   float* s_shift = s_scale + C;            // [C]
-  float* s_sum = s_shift + C;              // [C]
-  float* s_sq = s_sum + C;                 // [C]
+  float* s_psum = s_shift + C;             // with y_stats: [threads][8] per-thread sums, then [threads][8] squares
+  float* s_psq = s_psum + blockDim.x * 8;
   const int b = blockIdx.y, tid = threadIdx.x;
   const int c0 = blockIdx.z * C;            // this block's channel slice [c0, c0 + C) of the Ctot-channel layer
   const double nvox = (double)D * H * W;
@@ -82,7 +82,6 @@ __global__ void __launch_bounds__(256, 2) dwconv_fwd_kernel(DwArgs a) {
     if (a.x_stats) stats_to_mean_rstd(a.x_stats + ((int64_t)b * a.Ctot + c0 + c) * 2, nvox, a.eps, mean, rstd);
     // IN constants transposed [c%8][cg] for the same reason
     s_scale[(c & 7) * (C >> 3) + (c >> 3)] = rstd; s_shift[(c & 7) * (C >> 3) + (c >> 3)] = -mean * rstd;
-    s_sum[c] = 0.f; s_sq[c] = 0.f;
   }
   __syncthreads();
   const int ncg = C >> 3, WR = (W + RUN - 1) / RUN;
@@ -180,12 +179,20 @@ __global__ void __launch_bounds__(256, 2) dwconv_fwd_kernel(DwArgs a) {
     }
   }
   if (a.y_stats) {
-#pragma unroll
-    for (int c = 0; c < 8; ++c) { atomicAdd(&s_sum[cg * 8 + c], tsum[c]); atomicAdd(&s_sq[cg * 8 + c], tsq[c]); }
+    // thread tid = rl * ncg + cg parks its 8 channel partials at [tid * 8] = [rl * C + c]; each channel then sums its
+    // rl partials in order, so the block's contribution does not depend on warp timing (DESIGN §4a), and only the
+    // order of the fp64 atomics across blocks is free
+    *reinterpret_cast<float4*>(s_psum + tid * 8) = make_float4(tsum[0], tsum[1], tsum[2], tsum[3]);
+    *reinterpret_cast<float4*>(s_psum + tid * 8 + 4) = make_float4(tsum[4], tsum[5], tsum[6], tsum[7]);
+    *reinterpret_cast<float4*>(s_psq + tid * 8) = make_float4(tsq[0], tsq[1], tsq[2], tsq[3]);
+    *reinterpret_cast<float4*>(s_psq + tid * 8 + 4) = make_float4(tsq[4], tsq[5], tsq[6], tsq[7]);
     __syncthreads();
+    const int rb = blockDim.x / ncg;
     for (int c = tid; c < C; c += blockDim.x) {
+      float s = 0.f, q = 0.f;
+      for (int r = 0; r < rb; ++r) { s += s_psum[r * C + c]; q += s_psq[r * C + c]; }
       double* st = a.y_stats + ((int64_t)b * a.Ctot + c0 + c) * 2;
-      atomicAdd(st, (double)s_sum[c]); atomicAdd(st + 1, (double)s_sq[c]);
+      atomicAdd(st, (double)s); atomicAdd(st + 1, (double)q);
     }
   }
 }
@@ -320,7 +327,7 @@ extern "C" int b200seg_dwconv3d_fwd(const void* x, int x_ld, int x_coff, const d
   int cap = (B200SEG_NUM_SMS * 8 + B * nchunk - 1) / (B * nchunk);
   if (cap < 1) cap = 1;
   if (gx > cap) gx = cap;
-  const size_t sm = sizeof(float) * ((size_t)taps * chunk + 4 * chunk);
+  const size_t sm = sizeof(float) * ((size_t)taps * chunk + 2 * chunk + (y_stats ? 16 * (size_t)threads : 0));
   const int nr = !x_stats ? (act ? 3 : 0) : (act == 1 ? 2 : 1);
   const dim3 grid(gx, B, nchunk);
 #define B200_DW_FWD(TT, A, Bk, Ck, NRk) dwconv_fwd_kernel<TT, A, Bk, Ck, NRk><<<grid, threads, sm, st>>>(a)

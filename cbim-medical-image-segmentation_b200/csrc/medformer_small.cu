@@ -202,10 +202,14 @@ __global__ void se_gate_fwd_kernel(SeArgs a) {
 }
 
 // backward: every block recomputes dz2 (C) and dz1 (R, a C x R column reduction) and owns a slice of the C axis
-// for dw2/db2/dw1/dmean; block 0 also writes db1.  Each output element is touched by exactly one thread.
+// for dw2/db2/dw1/dmean; block 0 also writes db1.  Each output element is touched by exactly one thread, and every
+// partial sum is combined in a fixed order (per-warp / per-part partials in shared memory), so dz1 and dmean -- which
+// reach the SE input's gradient and everything upstream -- are the same on every run.
+constexpr int SE_RED = 16 * 256;           // [warps][256 r values] of the dz1 reduction; >= blockDim for dmean
 __global__ void se_gate_bwd_kernel(SeArgs a) {
   extern __shared__ float sm[];
   float* s_dz2 = sm; float* s_dz1 = sm + a.C; float* s_h = s_dz1 + a.R;     // [C], [R], [R]
+  float* s_red = s_h + a.R;                                                 // [SE_RED]
   const int tid = threadIdx.x;
   const int cper = (a.C + gridDim.x - 1) / gridDim.x, c0 = blockIdx.x * cper, c1 = min(a.C, c0 + cper);
   for (int b = 0; b < a.B; ++b) {
@@ -216,7 +220,7 @@ __global__ void se_gate_bwd_kernel(SeArgs a) {
     for (int r = tid; r < a.R; r += blockDim.x) { s_dz1[r] = 0.f; s_h[r] = a.hidden[b * a.R + r]; }
     __syncthreads();
     // dh[r] = sum_c w2[c][r] dz2[c]: a warp strides the c axis, its lanes hold up to 8 r values each (8 loads in
-    // flight per lane, coalesced along r); partials meet in shared memory
+    // flight per lane, coalesced along r); the per-warp partials are summed in warp order
     {
       const int lane = tid & 31, wid = tid >> 5, nw = blockDim.x >> 5;
       for (int rb = 0; rb < a.R; rb += 256) {
@@ -230,10 +234,16 @@ __global__ void se_gate_bwd_kernel(SeArgs a) {
           for (int u = 0; u < 8; ++u) if (rb + u * 32 + lane < a.R) acc[u] = fmaf(wr[u * 32], z, acc[u]);
         }
 #pragma unroll
-        for (int u = 0; u < 8; ++u) if (rb + u * 32 + lane < a.R) atomicAdd(&s_dz1[rb + u * 32 + lane], acc[u]);
+        for (int u = 0; u < 8; ++u) s_red[wid * 256 + u * 32 + lane] = acc[u];
+        __syncthreads();
+        for (int r = tid; r < 256 && rb + r < a.R; r += blockDim.x) {
+          float s = 0.f;
+          for (int w = 0; w < nw; ++w) s += s_red[w * 256 + r];
+          s_dz1[rb + r] = s;
+        }
+        __syncthreads();
       }
     }
-    __syncthreads();
     for (int r = tid; r < a.R; r += blockDim.x) {
       const float dz1 = s_h[r] > 0.f ? s_dz1[r] : 0.f;
       s_dz1[r] = dz1;
@@ -250,22 +260,23 @@ __global__ void se_gate_bwd_kernel(SeArgs a) {
       a.dw1[(int64_t)r * a.C + c] += s_dz1[r] * a.mean[b * a.C + c];
     }
     for (int c = c0 + tid; c < c1; c += blockDim.x) a.db2[c] += s_dz2[c];
-    // dmean[c] = sum_r w1[r][c] dz1[r] for the slice: threads (c, r-part), combined through shared memory
-    __syncthreads();
-    float* s_dm = s_dz2;                       // dz2 is no longer needed in this batch iteration
-    const int ncs = c1 - c0;
-    for (int c = tid; c < ncs; c += blockDim.x) s_dm[c] = 0.f;
-    __syncthreads();
+    // dmean[c] = sum_r w1[r][c] dz1[r] for the slice: threads (c, r-part), the parts summed in order
+    const int ncs = c1 - c0;                   // < blockDim: 132 blocks and the shared-memory cap keep C < 512 * 132
+    const int parts = ncs > 0 ? max(1, (int)blockDim.x / ncs) : 0;
     if (ncs > 0) {
-      const int parts = max(1, (int)blockDim.x / ncs), part = tid / ncs, cc = tid % ncs;
+      const int part = tid / ncs, cc = tid % ncs;
       if (part < parts) {
         float dm = 0.f;
         for (int r = part; r < a.R; r += parts) dm = fmaf(a.w1[(int64_t)r * a.C + c0 + cc], s_dz1[r], dm);
-        atomicAdd(&s_dm[cc], dm);
+        s_red[part * ncs + cc] = dm;
       }
     }
     __syncthreads();
-    for (int c = tid; c < ncs; c += blockDim.x) a.dmean[b * a.C + c0 + c] = s_dm[c];
+    for (int c = tid; c < ncs; c += blockDim.x) {
+      float s = 0.f;
+      for (int p = 0; p < parts; ++p) s += s_red[p * ncs + c];
+      a.dmean[b * a.C + c0 + c] = s;
+    }
     __syncthreads();
   }
 }
@@ -282,13 +293,12 @@ __global__ void scale_fwd_kernel(const T* x, const float* g, T* y, int64_t V, in
     st8<T>(y + vox * C + cg * 8, v);
   }
 }
-// dg[b][c] = sum_vox dy * x   (grid.y = b; block-level smem reduce, then one atomic per channel per block)
+// dg[b][c] = sum_vox dy * x in two passes that add in a fixed order (DESIGN §4a): grid (gx, B) blocks each write
+// the sum of their threads' partials to part[b][block][C]; the second pass adds the gx partials in block order.
 template <typename T>
-__global__ void scale_bwd_reduce_kernel(const T* dy, const T* x, float* dg, int64_t V, int C) {
-  extern __shared__ float s_acc[];
+__global__ void scale_bwd_reduce_kernel(const T* dy, const T* x, float* part, int64_t V, int C) {
+  extern __shared__ float s_part[];          // [threads][8]: thread tid = rl * ncg + cg at [rl * C + cg * 8]
   const int b = blockIdx.y, ncg = C >> 3, cg = threadIdx.x % ncg;
-  for (int c = threadIdx.x; c < C; c += blockDim.x) s_acc[c] = 0.f;
-  __syncthreads();
   float acc[8];
 #pragma unroll
   for (int c = 0; c < 8; ++c) acc[c] = 0.f;
@@ -300,9 +310,22 @@ __global__ void scale_bwd_reduce_kernel(const T* dy, const T* x, float* dg, int6
     for (int c = 0; c < 8; ++c) acc[c] = fmaf(g[c], v[c], acc[c]);
   }
 #pragma unroll
-  for (int c = 0; c < 8; ++c) atomicAdd(&s_acc[cg * 8 + c], acc[c]);
+  for (int c = 0; c < 8; ++c) s_part[threadIdx.x * 8 + c] = acc[c];
   __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) atomicAdd(&dg[b * C + c], s_acc[c]);
+  const int rb = blockDim.x / ncg;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float s = 0.f;
+    for (int r = 0; r < rb; ++r) s += s_part[r * C + c];
+    part[((int64_t)b * gridDim.x + blockIdx.x) * C + c] = s;
+  }
+}
+__global__ void scale_bwd_sum_kernel(const float* part, float* dg, int nblk, int C) {
+  const int b = blockIdx.y, c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const float* p = part + (int64_t)b * nblk * C + c;
+  float s = 0.f;
+  for (int k = 0; k < nblk; ++k) s += p[(int64_t)k * C];
+  dg[b * C + c] += s;
 }
 // dx = dy * g[b][c] + dmean[b][c] / V
 template <typename T>
@@ -578,13 +601,16 @@ extern "C" int b200seg_se_gate_bwd(const float* dgate, const float* gate, const 
   SeArgs a; memset(&a, 0, sizeof(a));
   a.dgate = dgate; a.gate = const_cast<float*>(gate); a.hidden = const_cast<float*>(hidden); a.mean = const_cast<float*>(mean);
   a.w1 = w1; a.w2 = w2; a.dw1 = dw1; a.db1 = db1; a.dw2 = dw2; a.db2 = db2; a.dmean = dmean; a.B = B; a.C = C; a.R = R;
-  se_gate_bwd_kernel<<<(C + 31) / 32 < B200SEG_NUM_SMS ? (C + 31) / 32 : B200SEG_NUM_SMS, 512, sizeof(float) * (C + 2 * R), as_stream(stream)>>>(a);
+  const size_t smem = sizeof(float) * ((size_t)C + 2 * (size_t)R + SE_RED);
+  if (smem > 200 * 1024) return B200SEG_EUNSUPPORTED;
+  B200_CUDA(cudaFuncSetAttribute(se_gate_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  se_gate_bwd_kernel<<<(C + 31) / 32 < B200SEG_NUM_SMS ? (C + 31) / 32 : B200SEG_NUM_SMS, 512, smem, as_stream(stream)>>>(a);
   B200_CHECK_LAUNCH("se_gate_bwd");
   return B200SEG_OK;
 }
 
 extern "C" int b200seg_channel_scale_fwd(const void* x, const float* gate, void* y, int B, int64_t V, int C, int dtype, void* stream) {
-  if (!x || !gate || !y || B <= 0 || V <= 0 || !ok_dtype(dtype)) return B200SEG_EINVAL;
+  if (!x || !gate || !y || B <= 0 || V <= 0 || C <= 0 || !ok_dtype(dtype)) return B200SEG_EINVAL;
   if (C % 8) return B200SEG_EUNSUPPORTED;
   const int64_t total = (int64_t)B * V * (C / 8);
   DISPATCH_T(dtype, scale_fwd_kernel<T><<<grid_for(total, 256), 256, 0, as_stream(stream)>>>((const T*)x, gate, (T*)y, V, C, total));
@@ -592,20 +618,36 @@ extern "C" int b200seg_channel_scale_fwd(const void* x, const float* gate, void*
   return B200SEG_OK;
 }
 
-extern "C" int b200seg_channel_scale_bwd_reduce(const void* dy, const void* x, float* dgate, int B, int64_t V, int C, int dtype, void* stream) {
-  if (!dy || !x || !dgate || B <= 0 || V <= 0 || !ok_dtype(dtype)) return B200SEG_EINVAL;
+// thread shape and block count of the first reduction pass; the workspace holds one [C] partial per (b, block)
+static int scale_bwd_shape(int64_t V, int C, int* threads) {
+  const int ncg = C / 8;
+  *threads = ncg >= 256 ? ncg : (256 / ncg) * ncg;
+  const int gx = grid_for(V * ncg, *threads);
+  return gx > 592 ? 592 : gx;
+}
+
+extern "C" size_t b200seg_channel_scale_bwd_workspace(int B, int64_t V, int C) {
+  if (B <= 0 || V <= 0 || C <= 0 || C % 8) return 0;
+  int threads;
+  return (size_t)B * scale_bwd_shape(V, C, &threads) * C * sizeof(float);
+}
+
+extern "C" int b200seg_channel_scale_bwd_reduce(const void* dy, const void* x, float* dgate, float* workspace, int B,
+                                                int64_t V, int C, int dtype, void* stream) {
+  if (!dy || !x || !dgate || !workspace || B <= 0 || V <= 0 || C <= 0 || !ok_dtype(dtype)) return B200SEG_EINVAL;
   if (C % 8 || C > 8192) return B200SEG_EUNSUPPORTED;
-  const int ncg = C / 8, threads = ncg >= 256 ? ncg : (256 / ncg) * ncg;
+  int threads;
+  const int gx = scale_bwd_shape(V, C, &threads);
   if (threads > 1024) return B200SEG_EUNSUPPORTED;
-  int gx = grid_for(V * ncg, threads);
-  if (gx > 592) gx = 592;
-  DISPATCH_T(dtype, scale_bwd_reduce_kernel<T><<<dim3(gx, B), threads, sizeof(float) * C, as_stream(stream)>>>((const T*)dy, (const T*)x, dgate, V, C));
+  cudaStream_t st = as_stream(stream);
+  DISPATCH_T(dtype, scale_bwd_reduce_kernel<T><<<dim3(gx, B), threads, sizeof(float) * 8 * threads, st>>>((const T*)dy, (const T*)x, workspace, V, C));
+  scale_bwd_sum_kernel<<<dim3((C + 255) / 256, B), 256, 0, st>>>(workspace, dgate, gx, C);
   B200_CHECK_LAUNCH("channel_scale_bwd_reduce");
   return B200SEG_OK;
 }
 
 extern "C" int b200seg_channel_scale_bwd_apply(const void* dy, const float* gate, const float* dmean, void* dx, int B, int64_t V, int C, int dtype, void* stream) {
-  if (!dy || !gate || !dx || B <= 0 || V <= 0 || !ok_dtype(dtype)) return B200SEG_EINVAL;
+  if (!dy || !gate || !dx || B <= 0 || V <= 0 || C <= 0 || !ok_dtype(dtype)) return B200SEG_EINVAL;
   if (C % 8) return B200SEG_EUNSUPPORTED;
   const int64_t total = (int64_t)B * V * (C / 8);
   DISPATCH_T(dtype, scale_bwd_apply_kernel<T><<<grid_for(total, 256), 256, 0, as_stream(stream)>>>((const T*)dy, gate, dmean, (T*)dx, V, C, total));

@@ -193,7 +193,9 @@ class SEScaleFn(torch.autograd.Function):
         R = s1[0]
         dev = x.device
         dgate = zeros_scratch((B, C), torch.float32, dev)
-        call("b200seg_channel_scale_bwd_reduce", dy.data_ptr(), x.data_ptr(), dgate.data_ptr(), B, V, C, _dt(x), _stream())
+        ws = torch.empty(_lib.load().b200seg_channel_scale_bwd_workspace(B, V, C), dtype=torch.uint8, device=dev)
+        call("b200seg_channel_scale_bwd_reduce", dy.data_ptr(), x.data_ptr(), dgate.data_ptr(), ws.data_ptr(), B, V, C,
+             _dt(x), _stream())
         dw1 = torch.zeros(R, C, dtype=torch.float32, device=dev)
         db1 = torch.zeros(R, dtype=torch.float32, device=dev)
         dw2 = torch.zeros(C, R, dtype=torch.float32, device=dev)

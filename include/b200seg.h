@@ -305,7 +305,8 @@ int b200seg_dwconv3d_wgrad(const void* x, int x_ld, int x_coff, const double* x_
  * se_gate: SEBlock conv_layers.py:159-174 on the channel means taken from IN
  *   sums: gate = sigmoid(W2 relu(W1 mean + b1) + b2); w1 [R][C], w2 [C][R].
  *   bwd accumulates (+=) dw1/db1/dw2/db2 and returns dmean.
- * channel_scale: y = x*gate[b][c]; bwd_reduce: dgate += sum_vox dy*x;
+ * channel_scale: y = x*gate[b][c]; bwd_reduce: dgate += sum_vox dy*x, added in a
+ *   fixed order through a float workspace of channel_scale_bwd_workspace bytes;
  *   bwd_apply: dx = dy*gate + dmean/V (dmean may be NULL).
  * layernorm: nn.LayerNorm(C, eps) trans_layers.py:36-41 over rows [R][C];
  *   mean_rstd float[R][2]; bwd accumulates (+=) dgamma/dbeta.
@@ -330,7 +331,8 @@ int b200seg_se_gate_bwd(const float* dgate, const float* gate, const float* hidd
                         const float* w1, const float* w2, float* dw1, float* db1, float* dw2, float* db2,
                         float* dmean, int B, int C, int R, void* stream);
 int b200seg_channel_scale_fwd(const void* x, const float* gate, void* y, int B, int64_t V, int C, int dtype, void* stream);
-int b200seg_channel_scale_bwd_reduce(const void* dy, const void* x, float* dgate, int B, int64_t V, int C, int dtype, void* stream);
+size_t b200seg_channel_scale_bwd_workspace(int B, int64_t V, int C);
+int b200seg_channel_scale_bwd_reduce(const void* dy, const void* x, float* dgate, float* workspace, int B, int64_t V, int C, int dtype, void* stream);
 int b200seg_channel_scale_bwd_apply(const void* dy, const float* gate, const float* dmean, void* dx, int B, int64_t V, int C, int dtype, void* stream);
 int b200seg_layernorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* mean_rstd,
                           int R, int C, float eps, int dtype, void* stream);
