@@ -17,12 +17,15 @@
 //     ([KC/8][NT][8] fp16): resident for the CTA's lifetime when the layer's weights fit (<=112 KB), else streamed
 //     by 1-D bulk TMA (cp.async.bulk) through an mbarrier ring.
 //   * D lives in the registers of two consumer warpgroups (64 rows each, wgmma m64 x NT x 16), which also run the
-//     epilogue: bias / residual / dgrad ReLU-mask, fp16 store, InstanceNorm sums of the stored tile.
+//     epilogue: bias / residual / dgrad ReLU-mask, fp16 store, InstanceNorm sums of the stored tile.  The epilogue's
+//     side operand (residual, or the pre-norm input of the dgrad mask) is one tensor-TMA box per tile in shared memory,
+//     issued a tile or more ahead, so no epilogue waits on a global load.
 // Warp roles (640 threads = 5 warpgroups, 1 CTA/SM, persistent over tiles; `setmaxnreg` moves registers from the
 // loader / weight warpgroups to the two consumer warpgroups, whose accumulators need them):
 //   warps 0-7  MMA + epilogue (warpgroup g = GEMM rows 64g .. 64g+63)
 //   warps 8-15 A loaders (cp.async / TMA + in-place transform; all 256 threads share every stage)
-//   warp  16   weight producer (bulk TMA); warps 17-19 only complete the warpgroup
+//   warp  16   weight producer (bulk TMA); warp 17 side-operand producer (tensor TMA); warps 18-19 only complete the
+//              warpgroup
 #include "common.cuh"
 #include "conv_args.h"
 #include "tc_common.cuh"
@@ -58,12 +61,15 @@ struct TcParams {
   int w_resident;          // all weights of the layer live in shared memory for the CTA's lifetime (no B ring)
   int prefetch;            // A stages the loaders keep in flight (1..3, < SA)
   int use_tma;             // halo tiles are staged by ONE tensor-TMA box per stage (else 16-byte cp.async copies)
-  int smem_a_off, smem_b_off, smem_bar_off, smem_norm_off, smem_gnorm_off;
+  int SS, side_stage_bytes; // side-operand slots (residual / dgrad_x tile, [NT/8 planes][128 voxels][8 ch]); 0 = none
+  int smem_a_off, smem_b_off, smem_side_off, smem_bar_off, smem_norm_off, smem_gnorm_off;
   alignas(64) CUtensorMap tm_x;      // x as {8 ch, w, h, channel plane, b*D + d}
+  alignas(64) CUtensorMap tm_side;   // res or gx (Cout channels), same dims; box {8, TW, TH, NT/8}
 };
 
-// barrier block layout (uint64 each): a_full[SA] a_empty[SA] b_full[SB] b_empty[SB] a_land[SA].  SA / SB are read from
-// the kernel parameters, not copied: copies would hold registers in every role (measured: more loader spills).
+// barrier block layout (uint64 each): a_full[SA] a_empty[SA] b_full[SB] b_empty[SB] a_land[SA] side_full[SS]
+// side_empty[SS].  SA / SB / SS are read from the kernel parameters, not copied: copies would hold registers in every
+// role (measured: more loader spills).
 struct Bars {
   uint32_t bar0; const TcParams& p;
   __device__ __forceinline__ uint32_t a_full(int i) const { return bar0 + 8u * (uint32_t)i; }
@@ -71,6 +77,8 @@ struct Bars {
   __device__ __forceinline__ uint32_t b_full(int i) const { return bar0 + 8u * (uint32_t)(2 * p.SA + i); }
   __device__ __forceinline__ uint32_t b_empty(int i) const { return bar0 + 8u * (uint32_t)(2 * p.SA + p.SB + i); }
   __device__ __forceinline__ uint32_t a_land(int i) const { return bar0 + 8u * (uint32_t)(2 * p.SA + 2 * p.SB + i); }   // TMA: the stage's box has landed
+  __device__ __forceinline__ uint32_t side_full(int i) const { return bar0 + 8u * (uint32_t)(3 * p.SA + 2 * p.SB + i); }
+  __device__ __forceinline__ uint32_t side_empty(int i) const { return bar0 + 8u * (uint32_t)(3 * p.SA + 2 * p.SB + p.SS + i); }
 };
 
 struct TileCoord { int b, d, h0, w0, ntile; };
@@ -355,7 +363,7 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
     }
   };
   if (resident) mbar_wait(bars.b_full(0), 0);
-  Ring ra, rb; ra.init(p.SA); rb.init(p.SB);
+  Ring ra, rb, rs; ra.init(p.SA); rb.init(p.SB); rs.init(p.SS);
   int pend_a = -1, pend_b = -1;                                        // slots read only by the group in flight
   auto release = [&]() {
     if (signaller) {
@@ -413,7 +421,6 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
 
     // ---- epilogue: bias / residual / dgrad mask, fp16 rounding and store, InstanceNorm sums
     const int co_base = tc.ntile * NT;
-    const __half* side[2];
     __half* yp[2];
     bool valid[2];
 #pragma unroll
@@ -422,9 +429,11 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
       valid[i] = h < a.H && w < a.W;
       const int64_t vox = ((int64_t)(tc.b * a.D + tc.d) * a.H + (valid[i] ? h : 0)) * a.W + (valid[i] ? w : 0);
       yp[i] = reinterpret_cast<__half*>(a.y) + vox * a.y_ld + a.y_coff + co_base;
-      side[i] = dgrad ? reinterpret_cast<const __half*>(a.gx) + vox * a.gx_ld + a.gx_coff + co_base
-                      : (a.res ? reinterpret_cast<const __half*>(a.res) + vox * a.r_ld + a.r_coff + co_base : nullptr);
     }
+    // side tile [NT/8 planes][128 rows][8 ch]: rows r0, r0 + 8 of plane j; the 8 lanes sharing a plane read 128
+    // consecutive bytes
+    const uint8_t* side = smem + p.smem_side_off + rs.idx * p.side_stage_bytes + r0 * 16 + 4 * (lane & 3);
+    if (has_side) mbar_wait(bars.side_full(rs.idx), rs.phase);
     const float2* gn = s_gnorm + tc.b * a.Cout + co_base;
     if (want_stats && tc.b * p.NTILES + tc.ntile != stat_key) { flush(); stat_key = tc.b * p.NTILES + tc.ntile; }
 #pragma unroll
@@ -438,7 +447,7 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
         if (!valid[i]) continue;                 // rows outside the volume: nothing stored, nothing counted
         float v0 = acc[4 * j + 2 * i] + bv.x, v1 = acc[4 * j + 2 * i + 1] + bv.y;
         float2 sv = make_float2(0.f, 0.f);
-        if (has_side) sv = __half22float2(*reinterpret_cast<const __half2*>(side[i] + c));
+        if (has_side) sv = __half22float2(*reinterpret_cast<const __half2*>(side + j * (TH * TW * 16) + i * 128));
         if (dgrad) {
           const float4 mr = *reinterpret_cast<const float4*>(gn + c);      // {mean, rstd} of two channels
           const float h0 = (sv.x - mr.x) * mr.y, h1 = (sv.y - mr.z) * mr.w;
@@ -461,6 +470,7 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
         if ((j & 7) == (lane >> 2)) { ks[j >> 3][0] += s0; ks[j >> 3][1] += s1; ks[j >> 3][2] += q0; ks[j >> 3][3] += q1; }
       }
     }
+    if (has_side) { mbar_arrive(bars.side_empty(rs.idx)); rs.advance(); }   // every consumer thread: its reads are done
   }
   if (want_stats) flush();
 }
@@ -487,6 +497,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   if (threadIdx.x == 0) {
     for (int i = 0; i < p.SA; ++i) { mbar_init(bars.a_full(i), kLoadThreads); mbar_init(bars.a_empty(i), kConsumerWGs); mbar_init(bars.a_land(i), 1); }
     for (int i = 0; i < p.SB; ++i) { mbar_init(bars.b_full(i), 1); mbar_init(bars.b_empty(i), kConsumerWGs); }
+    for (int i = 0; i < p.SS; ++i) { mbar_init(bars.side_full(i), 1); mbar_init(bars.side_empty(i), kConsumerWGs * 128); }
     fence_barrier_init();
   }
   {
@@ -546,6 +557,19 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
           }
         }
       }
+    } else if (warp == kWgtWarp + 1 && lane == 0 && p.SS > 0) {
+      // =========================== SIDE-OPERAND PRODUCER (tensor TMA) ===========================
+      // the residual / dgrad_x tile of every output tile, in tile order, up to SS tiles ahead of the epilogue
+      const uint32_t smem_side = smem_u32(smem + p.smem_side_off);
+      Ring ring; ring.init(p.SS);
+      TileWalk tw; tw.init(p); TileIter ti; ti.init(tw);
+      for (; ti.valid(tw); ti.next(tw)) {
+        mbar_wait(bars.side_empty(ring.idx), ring.phase ^ 1);
+        mbar_arrive_expect_tx(bars.side_full(ring.idx), (uint32_t)p.side_stage_bytes);
+        tma_load_5d(smem_side + (uint32_t)(ring.idx * p.side_stage_bytes), &p.tm_side, bars.side_full(ring.idx), 0, ti.wi * TW,
+                    ti.hi * TH, ti.ntile * (p.NT / 8), ti.b * a.D + ti.d);
+        ring.advance();
+      }
     }
   } else {
     // =========================== MMA + EPILOGUE (warps 0-7) ===========================
@@ -593,9 +617,11 @@ bool conv3d_fwd_tc_supported(const ConvArgs& a, int dtype) {
   if (a.res && ((a.r_ld % 8) || (a.r_coff % 8))) return false;
   if (a.gx && ((a.gx_ld % 8) || (a.gx_coff % 8))) return false;
   if ((reinterpret_cast<uintptr_t>(a.x) | reinterpret_cast<uintptr_t>(a.y) | reinterpret_cast<uintptr_t>(a.w)) & 15) return false;
+  // the residual / dgrad_x tile is a tensor-TMA box: 16-byte aligned base
+  if ((reinterpret_cast<uintptr_t>(a.res) | reinterpret_cast<uintptr_t>(a.gx)) & 15) return false;
   // The {mean, rstd} tables of x ([B][Cin], <= 32 KB) and, in dgrad mode, of dgrad_x ([B][Cout], <= 64 KB) live in
-  // shared memory; within these limits the planner in conv3d_fwd_tc still fits two A and two B stages of the largest
-  // tile.  (The InstanceNorm sums of y are kept in registers and need no table.)
+  // shared memory; within these limits the planner in conv3d_fwd_tc still fits the side-operand slots and two A and
+  // two B stages of the largest tile.  (The InstanceNorm sums of y are kept in registers and need no table.)
   if (a.B * a.Cin > 4096 || a.B * a.Cout > 8192) return false;
   return true;
 }
@@ -627,10 +653,22 @@ int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
   int64_t nt = (int64_t)a.B * a.D * p.tiles_h * p.tiles_w * p.NTILES;
   if (nt > 0x7fffffff) return B200SEG_EUNSUPPORTED;
   p.n_tiles = (int)nt;
+  // The epilogue's side operand (residual, or dgrad_x behind the activation mask) arrives as one tensor-TMA box
+  // {8 ch, TW, TH, NT/8 planes} per tile, zero-filled past the volume edge, in a ring of SS slots.  Narrow tiles
+  // (NT <= 64) take only a few hundred clocks of MMAs, so their box is issued two tiles ahead; wider tiles are long
+  // enough for one slot.
+  if (a.res || a.gx) {
+    p.SS = p.NT <= 64 ? 2 : 1;
+    p.side_stage_bytes = TH * TW * p.NT * 2;
+    const bool ok = a.gx ? b200seg_make_act_tmap(&p.tm_side, a.gx, a.gx_ld, a.gx_coff, a.Cout, a.B * a.D, a.H, a.W, TW, TH, p.NT / 8)
+                         : b200seg_make_act_tmap(&p.tm_side, a.res, a.r_ld, a.r_coff, a.Cout, a.B * a.D, a.H, a.W, TW, TH, p.NT / 8);
+    if (!ok) return B200SEG_ECUDA;       // conv3d_fwd_tc_supported checked every other condition of the map
+  }
   // shared memory carve-up
   const int norm_bytes = a.B * a.Cin * 8;
   const int gnorm_bytes = a.gx ? a.B * a.Cout * 8 : 0;
-  const int budget = 227 * 1024 - 1024 - norm_bytes - gnorm_bytes - 512;
+  const int side_bytes = p.SS * p.side_stage_bytes;
+  const int budget = 227 * 1024 - 1024 - norm_bytes - gnorm_bytes - side_bytes - 512;
   const int64_t w_total = (int64_t)a.kd * a.kh * a.kw * a.Cin * a.Cout * 2;
   int b_region;
   if (w_total <= 112 * 1024 && w_total + 2 * p.a_stage_bytes <= budget) {
@@ -652,8 +690,10 @@ int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
   p.smem_a_off = off; off += p.SA * p.a_stage_bytes;
   off = (off + 127) / 128 * 128;
   p.smem_b_off = off; off += b_region;
+  off = (off + 127) / 128 * 128;
+  p.smem_side_off = off; off += side_bytes;
   off = (off + 15) / 16 * 16;
-  p.smem_bar_off = off; off += (3 * p.SA + 2 * p.SB) * 8;
+  p.smem_bar_off = off; off += (3 * p.SA + 2 * p.SB + 2 * p.SS) * 8;
   off = (off + 15) / 16 * 16;
   p.smem_norm_off = off; off += norm_bytes;
   off = (off + 15) / 16 * 16;
