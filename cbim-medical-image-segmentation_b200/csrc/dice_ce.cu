@@ -6,7 +6,7 @@
 //   TP = sum P*M, SP = sum P, CNT = sum M  ->  FP = SP-TP, FN = CNT-TP
 //   alpha = clamp(FP/(FP+FN+s), .2, .8)  (kept in the autograd graph by the reference)
 //   dice  = TP / (TP + alpha FP + (1-alpha) FN + s);  Dice loss = mean_c (1 - dice)
-//   CE    = sum_v w[y] (lse - x_y) / sum_v w[y]
+//   CE    = sum_v w[y] (lse - x_y) / sum_v w[y]   (lse = m + log sum exp(x - m), m = max_c x)
 // Algorithmic bytes: fwd B*V*(C*s + label_bytes), bwd B*V*(2*C*s + label_bytes).
 #include "common.cuh"
 
@@ -87,23 +87,28 @@ dice_ce_fwd_kernel(const T* __restrict__ logits, int64_t stride_b, int64_t strid
     float x[C];
     load_logits<T, C, CL>(logits + b * stride_b + v * stride_v, stride_c, x);
     int y = load_label(labels, label_bytes, i);
-    float m = x[0];
+    float m = x[0], xy = 0.f;
 #pragma unroll
     for (int c = 1; c < C; ++c) m = fmaxf(m, x[c]);
+#pragma unroll
+    for (int c = 0; c < C; ++c) if (c == y) xy = x[c];
     float s = 0.f;
 #pragma unroll
     for (int c = 0; c < C; ++c) { x[c] = __expf(x[c] - m); s += x[c]; }
     float inv = 1.f / s;
-    float py = 0.f;
 #pragma unroll
     for (int c = 0; c < C; ++c) {
-      float p = x[c] * inv;
+      // rounded product, never fused into the sums: the Dice sums and with them the gradient stay bit-identical to
+      // the form that also kept p_y for the CE
+      float p = __fmul_rn(x[c], inv);
       sp[c] += p;
-      if (c == y) { tp[c] += p; cnt[c] += 1.f; py = p; }
+      if (c == y) { tp[c] += p; cnt[c] += 1.f; }
     }
     if (y >= 0 && y < C) {
+      // lse - x_y from the logits, not -log(p_y): p_y underflows in fp32 once x_y is ~88 below the max (fp16 logits
+      // reach 65504), while the CE of such a confidently wrong voxel keeps growing with the gap, as F.cross_entropy's
       float w = ce_w ? ce_w[y] : 1.f;
-      nll += w * (-__logf(fmaxf(py, 1e-30f)));
+      nll += w * ((m - xy) + logf(s));
       wsum += w;
     }
   }

@@ -188,7 +188,8 @@ upsample_fwd_kernel(const T* __restrict__ x, int x_ld, int x_coff, T* __restrict
 }
 
 // gather-form backward: each INPUT voxel collects from the output voxels whose stencil touches it
-// (deterministic, no atomics, no zero-fill).  Per axis at most kMaxTaps output indices contribute.
+// (deterministic, no atomics, no zero-fill).  Per axis at most kMaxTaps output indices contribute, except along an
+// input axis of length 1, which every output index reads (see AxisTab).
 constexpr int kMaxTaps = 12;
 __device__ __forceinline__ int axis_taps(float scale, int i, int in_size, int out_size, int (&oo)[kMaxTaps], float (&ww)[kMaxTaps]) {
   int n = 0;
@@ -212,9 +213,18 @@ __device__ __forceinline__ int axis_taps(float scale, int i, int in_size, int ou
 }
 
 // per-axis tap tables, built once per block in shared memory: for input index i the output indices whose
-// stencil touches i and their (non-zero) weights
+// stencil touches i and their (non-zero) weights.  An input axis of length 1 feeds every output index with weight 1,
+// however many there are: its single entry says so with n = -out_size instead of listing taps.
 struct AxisTab { int n; int o[kMaxTaps]; float w[kMaxTaps]; };
+__device__ __forceinline__ int tap_count(const AxisTab& t) { return t.n < 0 ? -t.n : t.n; }
+__device__ __forceinline__ int tap_out(const AxisTab& t, int k) { return t.n < 0 ? k : t.o[k]; }
+__device__ __forceinline__ float tap_w(const AxisTab& t, int k) { return t.n < 0 ? 1.f : t.w[k]; }
+
 __device__ __forceinline__ void build_axis_table(AxisTab* tab, float scale, int in_size, int out_size) {
+  if (in_size == 1) {
+    if (threadIdx.x == 0) tab[0].n = -out_size;
+    return;
+  }
   for (int i = threadIdx.x; i < in_size; i += kThreads) {
     int oo[kMaxTaps]; float ww[kMaxTaps];
     const int n = axis_taps(scale, i, in_size, out_size, oo, ww);
@@ -250,14 +260,15 @@ upsample_bwd_kernel(const T* __restrict__ dy, int dy_ld, int dy_coff, T* __restr
     float acc[VEC];
 #pragma unroll
     for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
-    for (int a = 0; a < ad.n; ++a)
-      for (int bq = 0; bq < ah.n; ++bq) {
-        const float wdh = ad.w[a] * ah.w[bq];
-        const T* row = dyb + (((int64_t)ad.o[a] * Ho + ah.o[bq]) * Wo) * dy_ld;
-        for (int c = 0; c < aw.n; ++c) {
+    const int nd = tap_count(ad), nh = tap_count(ah), nw = tap_count(aw);
+    for (int a = 0; a < nd; ++a)
+      for (int bq = 0; bq < nh; ++bq) {
+        const float wdh = tap_w(ad, a) * tap_w(ah, bq);
+        const T* row = dyb + (((int64_t)tap_out(ad, a) * Ho + tap_out(ah, bq)) * Wo) * dy_ld;
+        for (int c = 0; c < nw; ++c) {
           float g[VEC];
-          VecIO<VEC, T>::ld(row + (int64_t)aw.o[c] * dy_ld, g);
-          const float wt = wdh * aw.w[c];
+          VecIO<VEC, T>::ld(row + (int64_t)tap_out(aw, c) * dy_ld, g);
+          const float wt = wdh * tap_w(aw, c);
 #pragma unroll
           for (int i = 0; i < VEC; ++i) acc[i] += wt * g[i];
         }
@@ -365,7 +376,8 @@ extern "C" int b200seg_upsample_trilinear_bwd(const void* dy, int dy_ld, int dy_
   bool vok = vec_ok(dy, dy_ld, dy_coff, C) && vec_ok(dx, dx_ld, dx_coff, C);
   if (!vok && C > kThreads) return B200SEG_EUNSUPPORTED;
   float rd = host_scale(Di, Do), rh = host_scale(Hi, Ho), rw = host_scale(Wi, Wo);
-  // the gather needs every contributing output index to fit in kMaxTaps per axis
+  // the gather needs every contributing output index to fit in kMaxTaps per axis (a length-1 input axis, rd == 0
+  // with Di == 1, lists none: its table entry covers every output index)
   if ((Do > 1 && rd > 0.f && 2.0f / rd + 3.0f > (float)kMaxTaps && Do > kMaxTaps) ||
       (Ho > 1 && rh > 0.f && 2.0f / rh + 3.0f > (float)kMaxTaps && Ho > kMaxTaps) ||
       (Wo > 1 && rw > 0.f && 2.0f / rw + 3.0f > (float)kMaxTaps && Wo > kMaxTaps))

@@ -10,18 +10,25 @@ import torch.nn.functional as F
 SMOOTH = 1e-5
 
 
-def dice_loss(preds, targets):
-    """preds [B,C,...] float, targets [B,1,...] int64."""
-    C = preds.shape[1]
+def dice_terms(preds, targets):
+    """Per-class terms of dice_loss: (alpha before the clamp, alpha, dice), each [C]."""
     P = F.softmax(preds if preds.dtype == torch.float64 else preds.float(), dim=1)
     M = torch.zeros_like(P).scatter_(1, targets, 1.0)
     dims = [0] + list(range(2, P.dim()))           # batch and space jointly (losses.py:38-44)
     TP = (P * M).sum(dims)
     FP = (P * (1 - M)).sum(dims)
     FN = ((1 - P) * M).sum(dims)
-    alpha = torch.clamp(FP / (FP + FN + SMOOTH), min=0.2, max=0.8)
+    alpha_raw = FP / (FP + FN + SMOOTH)
+    alpha = torch.clamp(alpha_raw, min=0.2, max=0.8)
     beta = 1 - alpha
     dice = TP / (TP + alpha * FP + beta * FN + SMOOTH)
+    return alpha_raw, alpha, dice
+
+
+def dice_loss(preds, targets):
+    """preds [B,C,...] float, targets [B,1,...] int64."""
+    C = preds.shape[1]
+    dice = dice_terms(preds, targets)[2]
     return (1 - dice).sum() / C
 
 

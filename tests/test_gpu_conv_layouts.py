@@ -18,12 +18,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from util import global_l2, rel_err
+from util import assert_untouched, global_l2, rel_err, sentinel, wide
 
 pytestmark = pytest.mark.gpu
 
-POISON = 1000.0        # finite: an over-read multiplied by a zero weight must not turn into a false NaN failure
-SENTINEL = -777.0      # exact in fp16
 EPS = 1e-4
 TOL32, TOL16 = 1e-4, 4e-3
 
@@ -37,28 +35,6 @@ def lib():
 
 
 # ----------------------------------------------------------------------------- operands
-def wide(dense, ld, coff):
-    """dense [..., C] as channels coff .. coff+C of a [..., ld] buffer whose other channels hold +-POISON."""
-    C = dense.shape[-1]
-    assert coff + C <= ld
-    sign = 1.0 - 2.0 * (torch.arange(ld, device=dense.device) % 2)
-    buf = (POISON * sign).to(dense.dtype).expand(*dense.shape[:-1], ld).contiguous()
-    buf[..., coff:coff + C] = dense
-    return buf
-
-
-def sentinel(lead, ld, dtype):
-    return torch.full((*lead, ld), SENTINEL, dtype=dtype, device="cuda")
-
-
-def assert_untouched(buf, coff, C):
-    """the channels of an output buffer outside its slice still hold the sentinel, bit for bit"""
-    keep = torch.ones(buf.shape[-1], dtype=torch.bool, device=buf.device)
-    keep[coff:coff + C] = False
-    out = buf[..., keep]
-    assert torch.equal(out, torch.full_like(out, SENTINEL))
-
-
 def randh(*shape, dtype=torch.float16, scale=1.0, seed=0):
     g = torch.Generator().manual_seed(seed)
     return (torch.randn(*shape, generator=g) * scale).to(dtype).cuda()

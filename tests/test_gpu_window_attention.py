@@ -16,6 +16,7 @@ in dq cannot hide behind a larger dv).  fp16 rows compare with the reference rou
 rounds (bias, q * scale, probabilities)."""
 import ctypes
 import json
+import os
 import types
 
 import pytest
@@ -26,7 +27,7 @@ from oracle import swin_ops as so
 from oracle import swin_unetr as osw
 from oracle import unet3d as ounet
 from oracle.synth import make_volume
-from util import global_l2, rel_err
+from util import global_l2, launched_kernels_each, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -205,40 +206,64 @@ def _misaligned(t):
     return v
 
 
-def _kernels(fn):
-    """names of the window-attention kernels fn launches; fn runs once before the profiled call, so module loading and
-    the shared-memory attribute calls happen outside it.  The launches sit in a named range that starts with a torch op:
-    with nothing but the library's launches inside, a profiling session late in a long pytest process was seen to keep
-    only the last kernel."""
-    from torch.profiler import ProfilerActivity, profile, record_function
-    fn()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA], acc_events=True) as prof:
-        with record_function("window_attention"):
-            torch.zeros(16, device="cuda").add_(1)
-            fn()
-            torch.cuda.synchronize()
-    return sorted({e.name for e in prof.events() if "win_attn" in e.name})
+ROUTING_CASES = ["dh8", "dh16", "dh32", "dh4", "dh12", "dh24", "misaligned", "forced"]
+MIXED_ROWS = ["pad_shift", "clamp_w", "large_logit"]
+_NAMES = {}
+
+
+def _kernels(fn, arg):
+    """names of the window-attention kernels fn(arg) (_routing_launch or _mixed_launch) launches.  They are recorded by
+    the profiler in a fresh process, all cases in one: a profiling session late in a long pytest process was seen to
+    keep only the last kernel."""
+    if not _NAMES:
+        calls = [("_routing_launch", (c,)) for c in ROUTING_CASES] + [("_mixed_launch", (r,)) for r in MIXED_ROWS]
+        for call, names in zip(calls, launched_kernels_each("test_gpu_window_attention", calls)):
+            _NAMES[call] = sorted({n for n in names if "win_attn" in n})
+    return _NAMES[(fn, (arg,))]
+
+
+def _routing_inputs(case):
+    dh = int(case[2:]) if case.startswith("dh") else 16
+    dims, window, shift = GEOM["pad_shift"]
+    qkv, qb, table, dout = _inputs(dims, window, 3, dh, 2, seed=dh)
+    qkv, dout = qkv.half(), dout.half()
+    return dh, (window, shift), (qkv, qb, table, dout)
+
+
+def _routing_launch(case):
+    os.environ["B200SEG_WINATTN_MMA"] = "0" if case == "forced" else "1"      # a process of its own: no restore
+    _, (window, shift), (qkv, qb, table, dout) = _routing_inputs(case)
+    x = _misaligned(qkv) if case == "misaligned" else qkv
+    _raw(x, qb, table, dout, 3, window, shift)
+
+
+def _mixed_inputs(row):
+    dims, window, shift = GEOM[row]
+    qkv, qb, table, dout = _inputs(dims, window, 3, 16, 2, seed=31, **EXTRA.get(row, {}))
+    return (window, shift), (qkv.half(), qb, table, dout.half())
+
+
+def _mixed_launch(row):
+    os.environ["B200SEG_WINATTN_MMA"] = "1"
+    (window, shift), (qkv, qb, table, dout) = _mixed_inputs(row)
+    _raw(qkv, qb, table, _misaligned(dout), 3, window, shift)
 
 
 MMA_NAMES = ("win_attn_fwd_mma_kernel<%d>", "win_attn_bwd_q_mma_kernel<%d>", "win_attn_bwd_kv_mma_kernel<%d>")
 CC_NAMES = ("win_attn_fwd_kernel<__half>", "win_attn_bwd_q_kernel<__half>", "win_attn_bwd_kv_kernel<__half>")
 
 
-@pytest.mark.parametrize("case", ["dh8", "dh16", "dh32", "dh4", "dh12", "dh24", "misaligned", "forced"])
+@pytest.mark.parametrize("case", ROUTING_CASES)
 def test_kernel_routing(monkeypatch, case):
     """fp16 with dh 8 / 16 / 32 launches the tensor-core forward and both tensor-core backward passes; dh 4 / 12 / 24, a
     qkv that is not 16-byte aligned and B200SEG_WINATTN_MMA=0 launch the CUDA-core kernels (and still compute the
     operator)."""
-    dh = int(case[2:]) if case.startswith("dh") else 16
     monkeypatch.setenv("B200SEG_WINATTN_MMA", "0" if case == "forced" else "1")
-    dims, window, shift = GEOM["pad_shift"]
-    qkv, qb, table, dout = _inputs(dims, window, 3, dh, 2, seed=dh)
-    qkv, dout = qkv.half(), dout.half()
+    dh, (window, shift), (qkv, qb, table, dout) = _routing_inputs(case)
     x = _misaligned(qkv) if case == "misaligned" else qkv
-    res = {}
     # the raw entry points with fresh outputs, as WindowAttnFn calls them (dqkv is a new, aligned tensor)
-    names = _kernels(lambda: res.update(r=_raw(x, qb, table, dout, 3, window, shift)))
+    names = _kernels("_routing_launch", case)
+    res = {"r": _raw(x, qb, table, dout, 3, window, shift)}
     print(case, names)
     expect = [n % dh for n in MMA_NAMES] if case in ("dh8", "dh16", "dh32") else list(CC_NAMES)
     for e in expect:
@@ -249,17 +274,15 @@ def test_kernel_routing(monkeypatch, case):
     assert _err(res["r"][1], ref[1]) < BARS["fp16"][1]
 
 
-@pytest.mark.parametrize("row", ["pad_shift", "clamp_w", "large_logit"])
+@pytest.mark.parametrize("row", MIXED_ROWS)
 def test_mixed_paths(monkeypatch, row):
     """A dout that is not 16-byte aligned sends the backward to the CUDA cores after a tensor-core forward: the CUDA-core
     passes recompute P with an fp32 q * scale from an lse the tensor-core forward made with an fp16 one.  The result
     still meets the fp16 bars."""
     monkeypatch.setenv("B200SEG_WINATTN_MMA", "1")
-    dims, window, shift = GEOM[row]
-    qkv, qb, table, dout = _inputs(dims, window, 3, 16, 2, seed=31, **EXTRA.get(row, {}))
-    qkv, dout = qkv.half(), dout.half()
-    res = {}
-    names = _kernels(lambda: res.update(r=_raw(qkv, qb, table, _misaligned(dout), 3, window, shift)))
+    (window, shift), (qkv, qb, table, dout) = _mixed_inputs(row)
+    names = _kernels("_mixed_launch", row)
+    res = {"r": _raw(qkv, qb, table, _misaligned(dout), 3, window, shift)}
     assert len(names) == 3, names
     for e in (MMA_NAMES[0] % 16, CC_NAMES[1], CC_NAMES[2]):
         assert sum(e in n for n in names) == 1, (e, names)

@@ -5,12 +5,67 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
+POISON = 1000.0        # finite: an over-read multiplied by a zero weight must not turn into a false NaN failure
+SENTINEL = -777.0      # exact in fp16
+
+
+def wide(dense, ld, coff):
+    """dense [..., C] as channels coff .. coff+C of a [..., ld] buffer whose other channels hold +-POISON."""
+    C = dense.shape[-1]
+    assert coff + C <= ld
+    sign = 1.0 - 2.0 * (torch.arange(ld, device=dense.device) % 2)
+    buf = (POISON * sign).to(dense.dtype).expand(*dense.shape[:-1], ld).contiguous()
+    buf[..., coff:coff + C] = dense
+    return buf
+
+
+def sentinel(lead, ld, dtype):
+    return torch.full((*lead, ld), SENTINEL, dtype=dtype, device="cuda")
+
+
+def assert_untouched(buf, coff, C):
+    """the channels of an output buffer outside its slice still hold the sentinel, bit for bit"""
+    keep = torch.ones(buf.shape[-1], dtype=torch.bool, device=buf.device)
+    keep[coff:coff + C] = False
+    out = buf[..., keep]
+    assert torch.equal(out, torch.full_like(out, SENTINEL))
+
 
 def rel_err(a, b):
     """max-norm relative error: ||a-b||_inf / ||b||_inf (the parity metric of SURVEY.md §8d)."""
     a = a.detach().double().cpu()
     b = b.detach().double().cpu()
     return ((a - b).abs().max() / (b.abs().max() + 1e-30)).item()
+
+
+def launched_kernels(module, fn, *args):
+    """Names of the kernels `module.fn(*args)` launches (module: a test module; args: literals), recorded by
+    torch.profiler in a Python process of its own.  A profiling session late in a long pytest process can lose launches,
+    and each session makes that likelier for the next; in a fresh process the record is complete and the test process
+    is left as it was."""
+    return launched_kernels_each(module, [(fn, args)])[0]
+
+
+def launched_kernels_each(module, calls):
+    """launched_kernels for several (fn, args) calls of one module, one profiling session each, in one fresh process"""
+    import json
+    import subprocess
+    import sys
+    code = ("import json, sys\n"
+            "sys.path[:0] = [%r, %r]\n"
+            "import torch\n"
+            "from torch.profiler import ProfilerActivity, profile\n"
+            "import %s as m\n"
+            "out = []\n"
+            "for fn, args in %r:\n"
+            "    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA], acc_events=True) as prof:\n"
+            "        getattr(m, fn)(*args)\n"
+            "        torch.cuda.synchronize()\n"
+            "    out.append(sorted({e.name for e in prof.events()}))\n"
+            "print(json.dumps(out))\n") % (os.path.join(ROOT, "tests"), ROOT, module, [(f, tuple(a)) for f, a in calls])
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=200)
+    assert r.returncode == 0, r.stderr[-4000:]
+    return json.loads(r.stdout.strip().splitlines()[-1])
 
 
 def load_golden(name):
