@@ -448,8 +448,11 @@ int conv3d_fwd_small(const ConvArgs& a, int dtype, cudaStream_t st) {
   const bool plain = !a.x_stats && !a.act && !a.res && !a.gx;
   const bool k133 = (a.kd == 1 && a.kh == 3 && a.kw == 3), k333 = (a.kd == 3 && a.kh == 3 && a.kw == 3);
   const bool k111s = (a.kd == 1 && a.kh == 1 && a.kw == 1);
+  // stem_fwd_kernel stores y in 16-byte groups of 8 channels; pointwise_small_kernel moves x and y in 4-channel vectors
+  const uintptr_t xa = reinterpret_cast<uintptr_t>(a.x), ya = reinterpret_cast<uintptr_t>(a.y);
+  const uintptr_t vec4 = 4 * (dtype == B200SEG_F16 ? sizeof(__half) : sizeof(float));
   if (plain && !a.bias && a.Cin == 1 && (a.Cout == 32 || a.Cout == 48 || a.Cout == 64) && (k133 || k333 || k111s) && (a.y_ld % 8 == 0) &&
-      (a.y_coff % 8 == 0)) {
+      (a.y_coff % 8 == 0) && ya % 16 == 0) {
     dim3 grid(ceil_div(V, 256), a.B);
 #define STEM(TT, NG)                                                                   \
   do {                                                                                 \
@@ -466,7 +469,8 @@ int conv3d_fwd_small(const ConvArgs& a, int dtype, cudaStream_t st) {
   }
   const bool k111 = (a.kd == 1 && a.kh == 1 && a.kw == 1);
   if (plain && !a.y_stats && k111 && (a.Cin == 4 || a.Cin == 8 || a.Cin == 16 || a.Cin == 32 || a.Cin == 64) &&
-      a.Cout % 4 == 0 && a.Cout <= 64 && a.x_ld % 4 == 0 && a.x_coff % 4 == 0 && a.y_ld % 4 == 0 && a.y_coff % 4 == 0) {
+      a.Cout % 4 == 0 && a.Cout <= 64 && a.x_ld % 4 == 0 && a.x_coff % 4 == 0 && a.y_ld % 4 == 0 && a.y_coff % 4 == 0 &&
+      xa % vec4 == 0 && ya % vec4 == 0) {
     const int64_t total = (int64_t)a.B * V;
     const size_t sm = sizeof(float) * ((size_t)a.Cout * a.Cin + a.Cout);
     const int grid = ceil_div(total, 256);

@@ -48,21 +48,32 @@ def launched_kernels(module, fn, *args):
 
 def launched_kernels_each(module, calls):
     """launched_kernels for several (fn, args) calls of one module, one profiling session each, in one fresh process"""
+    code = ("from torch.profiler import ProfilerActivity, profile\n"
+            "out = []\n"
+            "for fn, args in %r:\n"
+            "    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA], acc_events=True) as prof:\n"
+            "        getattr(m, fn)(*args)\n"
+            "        torch.cuda.synchronize()\n"
+            "    out.append(sorted({e.name for e in prof.events()}))\n") % [(f, tuple(a)) for f, a in calls]
+    return _fresh(module, code)
+
+
+def run_fresh(module, fn, *args):
+    """module.fn(*args) (args: literals) in a Python process of its own; returns its JSON-serialisable result.  For
+    whole-model steps whose allocations and autograd state should not stay in the test process."""
+    return _fresh(module, "out = m.%s(*%r)\n" % (fn, tuple(args)))
+
+
+def _fresh(module, body):
     import json
     import subprocess
     import sys
     code = ("import json, sys\n"
             "sys.path[:0] = [%r, %r]\n"
             "import torch\n"
-            "from torch.profiler import ProfilerActivity, profile\n"
             "import %s as m\n"
-            "out = []\n"
-            "for fn, args in %r:\n"
-            "    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA], acc_events=True) as prof:\n"
-            "        getattr(m, fn)(*args)\n"
-            "        torch.cuda.synchronize()\n"
-            "    out.append(sorted({e.name for e in prof.events()}))\n"
-            "print(json.dumps(out))\n") % (os.path.join(ROOT, "tests"), ROOT, module, [(f, tuple(a)) for f, a in calls])
+            "%s"
+            "print(json.dumps(out))\n") % (os.path.join(ROOT, "tests"), ROOT, module, body)
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=200)
     assert r.returncode == 0, r.stderr[-4000:]
     return json.loads(r.stdout.strip().splitlines()[-1])
