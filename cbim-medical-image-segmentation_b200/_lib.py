@@ -39,6 +39,14 @@ _PROTOS = {
                            I, I, I, I, I, I, I, I, I, I, I, P],
     "b200seg_conv3d_wgrad_workspace": [I, I, I, I, I, I, I, I, I, I, I, I, I, I, I, I, I],
     "b200seg_conv3d_wgrad": [P, I, I, P, F, I, P, I, I, P, P, I, I, I, I, I, I, I, I, I, I, I, P, ctypes.c_size_t, P],
+    "b200seg_conv3d_fwd_pc": [P, I, I, P, I, P, P, P, I, I, P, I, I, P, I, I, I, I, I, I, I, I, I, I, I, P],
+    "b200seg_conv3d_wgrad_pc_workspace": [I, I, I, I, I, I, I, I, I, I, I, I, I, I, I, I, I],
+    "b200seg_conv3d_wgrad_pc": [P, I, I, P, I, P, I, I, P, P, I, I, I, I, I, I, I, I, I, I, I, P, ctypes.c_size_t, P],
+    "b200seg_batchnorm_fwd_fold": [P, I, I, c_double, P, P, P, P, P, F, F, I, P, P, P],
+    "b200seg_batchnorm_apply": [P, I, I, I, P, I, P, I, I, L, I, P],
+    "b200seg_batchnorm_bwd_reduce": [P, I, I, P, I, I, I, P, I, P, L, I, P, P],
+    "b200seg_batchnorm_bwd_fold": [P, c_double, P, P, I, I, P, P, P, P],
+    "b200seg_batchnorm_bwd_apply": [P, I, I, P, I, I, I, P, I, P, P, I, I, P, I, I, L, I, P],
     "b200seg_maxpool3d_fwd": [P, I, I, P, I, I, P, P, I, I, I, I, I, I, I, I, I, P],
     "b200seg_maxpool3d_bwd": [P, I, I, P, P, I, I, I, I, I, I, I, I, I, I, I, P],
     "b200seg_upsample_trilinear_fwd": [P, I, I, P, I, I, P, I, I, I, I, I, I, I, I, I, P],
@@ -88,7 +96,7 @@ _PROTOS = {
                            P, I, P, I, I, P, I, L, I, I, I, F, I, P],
 }
 _RESTYPES = {"b200seg_strerror": c_char_p, "b200seg_last_cuda_error": c_char_p,
-             "b200seg_conv3d_wgrad_workspace": ctypes.c_size_t, "b200seg_biattn_workspace": ctypes.c_size_t,
+             "b200seg_conv3d_wgrad_workspace": ctypes.c_size_t, "b200seg_conv3d_wgrad_pc_workspace": ctypes.c_size_t, "b200seg_biattn_workspace": ctypes.c_size_t,
              "b200seg_mapgen_workspace": ctypes.c_size_t,
              "b200seg_channel_scale_bwd_workspace": ctypes.c_size_t, "b200seg_window_attn_workspace": ctypes.c_size_t,
              "b200seg_surface_distance_workspace": ctypes.c_size_t}

@@ -70,6 +70,27 @@ extern "C" int b200seg_conv3d_fwd(const void* x, int x_ld, int x_coff, const dou
   return conv3d_fwd_direct(a, dtype, st);
 }
 
+// Per-channel (BatchNorm) mode: x enters as act(x*s[c] + t[c]) from the [Cin][2] table x_affine (nullptr: act(x)).  The
+// table is one row for the whole batch, so the tensor-core limits are those of B = 1 (b200seg_conv3d_algo(..., 1)).
+extern "C" int b200seg_conv3d_fwd_pc(const void* x, int x_ld, int x_coff, const float* x_affine, int act,
+                                     const void* w_packed, const float* bias, const void* residual, int r_ld, int r_coff,
+                                     void* y, int y_ld, int y_coff, double* y_stats, int B, int D, int H, int W,
+                                     int Cin, int Cout, int kd, int kh, int kw, int dtype, int algo, void* stream) {
+  if (!x || !w_packed || !y || B <= 0 || D <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0) return B200SEG_EINVAL;
+  if (kd <= 0 || kh <= 0 || kw <= 0 || !(kd & 1) || !(kh & 1) || !(kw & 1)) return B200SEG_EUNSUPPORTED;
+  if (dtype != B200SEG_F16 && dtype != B200SEG_F32) return B200SEG_EINVAL;
+  ConvArgs a{x, x_ld, x_coff, nullptr, 0.f, act, w_packed, bias, residual, r_ld, r_coff, y, y_ld, y_coff, y_stats,
+             nullptr, 0, 0, nullptr, 0.f, 0, B, D, H, W, Cin, Cout, kd, kh, kw, x_affine, 1};
+  cudaStream_t st = as_stream(stream);
+  if (algo == B200SEG_ALGO_TC) return conv3d_fwd_tc(a, dtype, st);
+  if (algo != B200SEG_ALGO_DIRECT) return B200SEG_EINVAL;
+  {
+    const int rc = conv3d_fwd_small(a, dtype, st);
+    if (rc != B200SEG_EUNSUPPORTED) return rc;
+  }
+  return conv3d_fwd_direct(a, dtype, st);
+}
+
 
 // ---- bias gradient db[c] += sum_v dy[v][c] as its own column-sum pass, so that convolutions / Linears WITH a bias
 // (every nn.Linear of SwinUNETR: qkv, proj, fc1, fc2 — 32 per step) can take the tensor-core weight-gradient kernel, which has
@@ -145,18 +166,9 @@ static int wgrad_args(WgradArgs& a, const void* x, int x_ld, int x_coff, const d
   return B200SEG_OK;
 }
 
-extern "C" size_t b200seg_conv3d_wgrad_workspace(int x_ld, int x_coff, int normalised, int dy_ld, int dy_coff,
-                                                 int want_bias, int B, int D, int H, int W, int Cin, int Cout,
-                                                 int kd, int kh, int kw, int dtype, int algo) {
-  WgradArgs a;
-  static const double dummy_stats = 0.0;
-  static float dummy_bias = 0.f;
-  // 16-byte aligned placeholders stand in for the tensors (only shapes/strides decide)
-  if (wgrad_args(a, (const void*)16, x_ld, x_coff, normalised ? &dummy_stats : nullptr, 1e-4f, normalised ? 1 : 0,
-                 (const void*)16, dy_ld, dy_coff, (float*)16, want_bias ? &dummy_bias : nullptr, B, D, H, W, Cin, Cout,
-                 kd, kh, kw, dtype)) return 0;
-  // covers every path b200seg_conv3d_wgrad can take for this shape: the real tensors' alignment (the placeholders here
-  // are aligned) can only rule the tensor-core path out, and then the special kernel or the CUDA-core path runs
+static size_t wgrad_workspace(const WgradArgs& a, int dtype, int algo) {
+  // covers every path b200seg_conv3d_wgrad can take for this shape: the real tensors' alignment (the placeholders of
+  // the callers are aligned) can only rule the tensor-core path out, and then the special kernel or the CUDA-core path runs
   if (algo == B200SEG_ALGO_DIRECT) return 0;
   if (algo == B200SEG_ALGO_TC) return conv3d_wgrad_tc_supported(a, dtype) ? conv3d_wgrad_tc_workspace(a) : 0;
   size_t ws = conv3d_wgrad_small_workspace(a), tc = 0;
@@ -169,15 +181,34 @@ extern "C" size_t b200seg_conv3d_wgrad_workspace(int x_ld, int x_coff, int norma
   return tc > ws ? tc : ws;
 }
 
-extern "C" int b200seg_conv3d_wgrad(const void* x, int x_ld, int x_coff, const double* x_stats, float eps, int act,
-                                    const void* dy, int dy_ld, int dy_coff, float* dw, float* dbias, int B, int D,
-                                    int H, int W, int Cin, int Cout, int kd, int kh, int kw, int dtype, int algo,
-                                    void* workspace, size_t ws_bytes, void* stream) {
-  if (!x || !dy || !dw) return B200SEG_EINVAL;
+extern "C" size_t b200seg_conv3d_wgrad_workspace(int x_ld, int x_coff, int normalised, int dy_ld, int dy_coff,
+                                                 int want_bias, int B, int D, int H, int W, int Cin, int Cout,
+                                                 int kd, int kh, int kw, int dtype, int algo) {
   WgradArgs a;
-  int rc = wgrad_args(a, x, x_ld, x_coff, x_stats, eps, act, dy, dy_ld, dy_coff, dw, dbias, B, D, H, W, Cin, Cout, kd, kh, kw, dtype);
-  if (rc) return rc;
-  cudaStream_t st = as_stream(stream);
+  static const double dummy_stats = 0.0;
+  static float dummy_bias = 0.f;
+  // 16-byte aligned placeholders stand in for the tensors (only shapes/strides decide)
+  if (wgrad_args(a, (const void*)16, x_ld, x_coff, normalised ? &dummy_stats : nullptr, 1e-4f, normalised ? 1 : 0,
+                 (const void*)16, dy_ld, dy_coff, (float*)16, want_bias ? &dummy_bias : nullptr, B, D, H, W, Cin, Cout,
+                 kd, kh, kw, dtype)) return 0;
+  return wgrad_workspace(a, dtype, algo);
+}
+
+extern "C" size_t b200seg_conv3d_wgrad_pc_workspace(int x_ld, int x_coff, int transformed, int dy_ld, int dy_coff,
+                                                    int want_bias, int B, int D, int H, int W, int Cin, int Cout,
+                                                    int kd, int kh, int kw, int dtype, int algo) {
+  WgradArgs a;
+  static const float dummy_affine[2] = {1.f, 0.f};
+  static float dummy_bias = 0.f;
+  if (wgrad_args(a, (const void*)16, x_ld, x_coff, nullptr, 0.f, transformed ? 1 : 0, (const void*)16, dy_ld, dy_coff,
+                 (float*)16, want_bias ? &dummy_bias : nullptr, B, D, H, W, Cin, Cout, kd, kh, kw, dtype)) return 0;
+  a.x_affine = transformed ? dummy_affine : nullptr;
+  a.per_channel = 1;
+  return wgrad_workspace(a, dtype, algo);
+}
+
+static int wgrad_dispatch(WgradArgs& a, int dtype, int algo, void* workspace, size_t ws_bytes, cudaStream_t st) {
+  int rc;
   if (algo == B200SEG_ALGO_TC) return conv3d_wgrad_tc(a, dtype, workspace, ws_bytes, st);
   if (algo == B200SEG_ALGO_AUTO && conv3d_wgrad_tc_supported(a, dtype))
     return conv3d_wgrad_tc(a, dtype, workspace, ws_bytes, st);
@@ -203,4 +234,29 @@ extern "C" int b200seg_conv3d_wgrad(const void* x, int x_ld, int x_coff, const d
     if (rc != B200SEG_EUNSUPPORTED) return rc;
   }
   return conv3d_wgrad_direct(a, dtype, st);
+}
+
+extern "C" int b200seg_conv3d_wgrad(const void* x, int x_ld, int x_coff, const double* x_stats, float eps, int act,
+                                    const void* dy, int dy_ld, int dy_coff, float* dw, float* dbias, int B, int D,
+                                    int H, int W, int Cin, int Cout, int kd, int kh, int kw, int dtype, int algo,
+                                    void* workspace, size_t ws_bytes, void* stream) {
+  if (!x || !dy || !dw) return B200SEG_EINVAL;
+  WgradArgs a;
+  int rc = wgrad_args(a, x, x_ld, x_coff, x_stats, eps, act, dy, dy_ld, dy_coff, dw, dbias, B, D, H, W, Cin, Cout, kd, kh, kw, dtype);
+  if (rc) return rc;
+  return wgrad_dispatch(a, dtype, algo, workspace, ws_bytes, as_stream(stream));
+}
+
+// Per-channel (BatchNorm) mode of the weight gradient: x enters as act(x*s[c] + t[c]) (see b200seg_conv3d_fwd_pc).
+extern "C" int b200seg_conv3d_wgrad_pc(const void* x, int x_ld, int x_coff, const float* x_affine, int act,
+                                       const void* dy, int dy_ld, int dy_coff, float* dw, float* dbias, int B, int D,
+                                       int H, int W, int Cin, int Cout, int kd, int kh, int kw, int dtype, int algo,
+                                       void* workspace, size_t ws_bytes, void* stream) {
+  if (!x || !dy || !dw) return B200SEG_EINVAL;
+  WgradArgs a;
+  int rc = wgrad_args(a, x, x_ld, x_coff, nullptr, 0.f, act, dy, dy_ld, dy_coff, dw, dbias, B, D, H, W, Cin, Cout, kd, kh, kw, dtype);
+  if (rc) return rc;
+  a.x_affine = x_affine;
+  a.per_channel = 1;
+  return wgrad_dispatch(a, dtype, algo, workspace, ws_bytes, as_stream(stream));
 }

@@ -12,6 +12,10 @@ struct ConvArgs {
   void* y; int y_ld, y_coff; double* y_stats;
   const void* gx; int gx_ld, gx_coff; const double* g_stats; float g_eps; int g_act;
   int B, D, H, W, Cin, Cout, kd, kh, kw;
+  // Per-channel input transform (BatchNorm): x is replaced by act(x*s[c] + t[c]) from the [Cin][2] {s, t} table
+  // x_affine (nullptr: act(x) only).  In this mode x_stats and the data-gradient mask are not used, and the shared
+  // table is [Cin] for any batch size.
+  const float* x_affine; int per_channel;
 };
 
 struct WgradArgs {
@@ -21,6 +25,7 @@ struct WgradArgs {
   int B, D, H, W, Cin, Cout, kd, kh, kw;
   int vox_per_block;
   float* part;         // per-block partial slices (conv3d_wgrad_small_workspace bytes), summed in block order
+  const float* x_affine; int per_channel;     // as in ConvArgs
 };
 
 int conv3d_fwd_direct(const ConvArgs& a, int dtype, cudaStream_t st);

@@ -43,9 +43,12 @@ conv_fwd_direct_kernel(ConvArgs a) {
   if (valid) { w0 = (int)(v % a.W); int64_t t = v / a.W; h0 = (int)(t % a.H); d0 = (int)(t / a.H); }
 
   const bool norm = a.x_stats != nullptr;
+  const bool affine = a.x_affine != nullptr;        // per-channel transform: s_mean holds the scale, s_rstd the shift
   if (norm) {
     for (int c = threadIdx.x; c < a.Cin; c += kVoxTile)
       stats_to_mean_rstd(a.x_stats + ((int64_t)b * a.Cin + c) * 2, (double)V, a.eps, s_mean[c], s_rstd[c]);
+  } else if (affine) {
+    for (int c = threadIdx.x; c < a.Cin; c += kVoxTile) { s_mean[c] = a.x_affine[2 * c]; s_rstd[c] = a.x_affine[2 * c + 1]; }
   }
   const T* xb = (const T*)a.x + (int64_t)b * V * a.x_ld + a.x_coff;
   const T* wp = (const T*)a.w;
@@ -78,6 +81,9 @@ conv_fwd_direct_kernel(ConvArgs a) {
             if (norm) {
 #pragma unroll
               for (int j = 0; j < CIV; ++j) xv[j] = (xv[j] - s_mean[ci0 + j]) * s_rstd[ci0 + j];
+            } else if (affine) {
+#pragma unroll
+              for (int j = 0; j < CIV; ++j) xv[j] = fmaf(xv[j], s_mean[ci0 + j], s_rstd[ci0 + j]);
             }
             if (a.act) {
 #pragma unroll
@@ -169,7 +175,7 @@ conv_wgrad_direct_kernel(WgradArgs a) {
   const int64_t v0 = (int64_t)blockIdx.x * a.vox_per_block;
   int64_t v1 = v0 + a.vox_per_block; if (v1 > V) v1 = V;
   const int zd = tap / (a.kh * a.kw) - a.kd / 2, zh = (tap / a.kw) % a.kh - a.kh / 2, zw = tap % a.kw - a.kw / 2;
-  const bool norm = a.x_stats != nullptr;
+  const bool norm = a.x_stats != nullptr, affine = a.x_affine != nullptr;
   const T* xb = (const T*)a.x + (int64_t)b * V * a.x_ld + a.x_coff;
   const T* dyb = (const T*)a.dy + (int64_t)b * V * a.dy_ld + a.dy_coff;
 
@@ -181,6 +187,8 @@ conv_wgrad_direct_kernel(WgradArgs a) {
   float mean = 0.f, rstd = 1.f;
   if (norm && ci0 + lc < a.Cin)
     stats_to_mean_rstd(a.x_stats + ((int64_t)b * a.Cin + ci0 + lc) * 2, (double)V, a.eps, mean, rstd);
+  float scale = 1.f, shift = 0.f;
+  if (affine && ci0 + lc < a.Cin) { scale = a.x_affine[2 * (ci0 + lc)]; shift = a.x_affine[2 * (ci0 + lc) + 1]; }
 
   for (int64_t vb = v0; vb < v1; vb += kWV) {
     __syncthreads();
@@ -198,6 +206,7 @@ conv_wgrad_direct_kernel(WgradArgs a) {
           if ((unsigned)d < (unsigned)a.D && (unsigned)h < (unsigned)a.H && (unsigned)w < (unsigned)a.W) {
             av = Elem<T>::ld(xb + (((int64_t)d * a.H + h) * a.W + w) * a.x_ld + ci0 + lc);
             if (norm) av = (av - mean) * rstd;
+            else if (affine) av = fmaf(av, scale, shift);
             av = act_apply(av, a.act);
             av = Elem<T>::round(av);
           }

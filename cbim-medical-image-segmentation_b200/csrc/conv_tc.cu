@@ -63,6 +63,7 @@ struct TcParams {
   int use_tma;             // halo tiles are staged by ONE tensor-TMA box per stage (else 16-byte cp.async copies)
   int SS, side_stage_bytes; // side-operand slots (residual / dgrad_x tile, [NT/8 planes][128 voxels][8 ch]); 0 = none
   int smem_a_off, smem_b_off, smem_side_off, smem_bar_off, smem_norm_off, smem_gnorm_off;
+  int norm_bstride;        // entries per sample in the {scale, shift} table: Cin, or 0 for a per-channel table
   alignas(64) CUtensorMap tm_x;      // x as {8 ch, w, h, channel plane, b*D + d}
   alignas(64) CUtensorMap tm_side;   // res or gx (Cout channels), same dims; box {8, TW, TH, NT/8}
 };
@@ -154,7 +155,7 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
   const bool active = lt < vstep * cpv;
   const int c8 = lt % cpv, v0 = lt / cpv;
   const int ph = a.kh / 2, pw = a.kw / 2;
-  const bool xform = (a.x_stats != nullptr) || (a.act != 0);
+  const bool xform = (a.x_stats != nullptr) || (a.x_affine != nullptr) || (a.act != 0);
   const int act = a.act;
   const __half* xbase = reinterpret_cast<const __half*>(a.x);
   const uint32_t smem_a = smem_u32(smem + p.smem_a_off) + (uint32_t)(c8 * p.plane_stride);
@@ -215,7 +216,7 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
 
   const float slope = act_slope(act);
   const bool relu = act == B200SEG_ACT_RELU;
-  float sc[8], sf[8];                              // x*sc + sf == (x - mean) * rstd for this thread's 8 channels
+  float sc[8], sf[8];                              // x*sc + sf: (x - mean) * rstd, or the per-channel affine transform
   int norm_key = -1;                               // (b, kc) the constants belong to
 #pragma unroll
   for (int i = 0; i < P; ++i) { if (ci.valid(tw)) issue(); if constexpr (!TMA) cp_async_commit(); }
@@ -228,8 +229,8 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
         norm_key = key;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          const float2 mr = s_norm[cd.ti.b * a.Cin + cd.kc * p.KC + c8 * 8 + j];
-          sc[j] = mr.y; sf[j] = -mr.x * mr.y;
+          const float2 st = s_norm[cd.ti.b * p.norm_bstride + cd.kc * p.KC + c8 * 8 + j];
+          sc[j] = st.x; sf[j] = st.y;
         }
       }
       uint8_t* sp = TMA ? smem + p.smem_a_off + rd.idx * p.a_stage_bytes : smem_a_gen + rd.idx * p.a_stage_bytes + v0 * 16;
@@ -324,7 +325,7 @@ template <int NT, int KSTEPS>
 __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid, uint8_t* smem, const Bars& bars, const float2* s_gnorm) {
   const ConvArgs& a = p.a;
   // A stage ready: published by the loaders, or (raw input staged by TMA) the TMA's own transaction barrier
-  const uint32_t a_ready0 = (p.use_tma && !(a.x_stats || a.act)) ? bars.a_land(0) : bars.a_full(0);
+  const uint32_t a_ready0 = (p.use_tma && !(a.x_stats || a.x_affine || a.act)) ? bars.a_land(0) : bars.a_full(0);
   const int warp = tid >> 5, lane = tid & 31;
   const bool signaller = tid == 0;
   const int r0 = 64 * wg + 16 * warp + (lane >> 2);
@@ -489,7 +490,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   const int pd = a.kd / 2;
   const Bars bars{smem_u32(smem + p.smem_bar_off), p};
 
-  float2* s_norm = reinterpret_cast<float2*>(smem + p.smem_norm_off);   // [B][Cin] {mean, rstd}
+  float2* s_norm = reinterpret_cast<float2*>(smem + p.smem_norm_off);   // [B or 1][Cin] {scale, shift} of x
   float2* s_gnorm = reinterpret_cast<float2*>(smem + p.smem_gnorm_off); // [B][Cout] {mean, rstd} of dgrad_x
   const uint32_t smem_b = smem_u32(smem + p.smem_b_off);
 
@@ -502,10 +503,14 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   }
   {
     const double n = (double)a.D * a.H * a.W;
-    for (int i = threadIdx.x; i < a.B * a.Cin; i += kThreads) {
-      float m = 0.f, r = 1.f;
-      if (a.x_stats) stats_to_mean_rstd(a.x_stats + (int64_t)i * 2, n, a.eps, m, r);
-      s_norm[i] = make_float2(m, r);
+    for (int i = threadIdx.x; i < (a.per_channel ? 1 : a.B) * a.Cin; i += kThreads) {
+      if (a.x_affine) {
+        s_norm[i] = make_float2(a.x_affine[2 * i], a.x_affine[2 * i + 1]);
+      } else {
+        float m = 0.f, r = 1.f;
+        if (a.x_stats) stats_to_mean_rstd(a.x_stats + (int64_t)i * 2, n, a.eps, m, r);
+        s_norm[i] = make_float2(r, -m * r);
+      }
     }
     if (a.gx) {
       for (int i = threadIdx.x; i < a.B * a.Cout; i += kThreads) {
@@ -520,7 +525,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   if (warp >= kLoadWarp0 && warp < kWgtWarp) {
     // =========================== A LOADERS ===========================
     setmaxnreg_dec<kRegsLoad>();
-    if (p.use_tma && !(a.x_stats || a.act)) loader_role_tma(p, smem, bars);
+    if (p.use_tma && !(a.x_stats || a.x_affine || a.act)) loader_role_tma(p, smem, bars);
     else if (p.use_tma) loader_role<3, true>(p, smem, s_norm, bars);
     else if (p.prefetch >= 3) loader_role<3, false>(p, smem, s_norm, bars);
     else loader_role<1, false>(p, smem, s_norm, bars);
@@ -619,10 +624,12 @@ bool conv3d_fwd_tc_supported(const ConvArgs& a, int dtype) {
   if ((reinterpret_cast<uintptr_t>(a.x) | reinterpret_cast<uintptr_t>(a.y) | reinterpret_cast<uintptr_t>(a.w)) & 15) return false;
   // the residual / dgrad_x tile is a tensor-TMA box: 16-byte aligned base
   if ((reinterpret_cast<uintptr_t>(a.res) | reinterpret_cast<uintptr_t>(a.gx)) & 15) return false;
-  // The {mean, rstd} tables of x ([B][Cin], <= 32 KB) and, in dgrad mode, of dgrad_x ([B][Cout], <= 64 KB) live in
-  // shared memory; within these limits the planner in conv3d_fwd_tc still fits the side-operand slots and two A and
-  // two B stages of the largest tile.  (The InstanceNorm sums of y are kept in registers and need no table.)
-  if (a.B * a.Cin > 4096 || a.B * a.Cout > 8192) return false;
+  // The transform table of x ([B][Cin], or [Cin] in per-channel mode, <= 32 KB) and, in dgrad mode, the {mean, rstd}
+  // table of dgrad_x ([B][Cout], <= 64 KB) live in shared memory; within these limits the planner in conv3d_fwd_tc
+  // still fits the side-operand slots and two A and two B stages of the largest tile.  (The InstanceNorm sums of y are
+  // kept in registers and need no table.)
+  const int nb = a.per_channel ? 1 : a.B;
+  if (nb * a.Cin > 4096 || nb * a.Cout > 8192) return false;
   return true;
 }
 
@@ -642,7 +649,7 @@ int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
   // box per stage and consumed by the MMA warpgroups straight off the TMA barrier; inputs that need InstanceNorm /
   // activation by a TMA box + in-place transform while Cin <= 64 and at least 4 A stages fit (below), by per-thread
   // cp.async copies + transform otherwise.  When the tensor map cannot be built every input takes the cp.async path.
-  const bool raw_input = !a.x_stats && a.act == 0;
+  const bool raw_input = !a.x_stats && !a.x_affine && a.act == 0;
   p.use_tma = ((raw_input || a.Cin <= 64) &&
                b200seg_make_act_tmap(&p.tm_x, a.x, a.x_ld, a.x_coff, a.Cin, a.B * a.D, a.H, a.W, p.HALO_W, p.HALO_H, p.KC / 8)) ? 1 : 0;
   p.plane_stride = p.use_tma ? p.nvox_h * 16 : slots * 16;    // a TMA box is written densely
@@ -665,7 +672,8 @@ int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
     if (!ok) return B200SEG_ECUDA;       // conv3d_fwd_tc_supported checked every other condition of the map
   }
   // shared memory carve-up
-  const int norm_bytes = a.B * a.Cin * 8;
+  p.norm_bstride = a.per_channel ? 0 : a.Cin;
+  const int norm_bytes = (a.per_channel ? 1 : a.B) * a.Cin * 8;
   const int gnorm_bytes = a.gx ? a.B * a.Cout * 8 : 0;
   const int side_bytes = p.SS * p.side_stage_bytes;
   const int budget = 227 * 1024 - 1024 - norm_bytes - gnorm_bytes - side_bytes - 512;

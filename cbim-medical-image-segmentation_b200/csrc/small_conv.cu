@@ -245,6 +245,7 @@ int small_wgrad_kind(const WgradArgs& a) {
   const int taps = a.kd * a.kh * a.kw;
   const bool k133 = (a.kd == 1 && a.kh == 3 && a.kw == 3), k333 = (a.kd == 3 && a.kh == 3 && a.kw == 3);
   const bool k111 = taps == 1;         // the 1x1x1 projection of SwinUNETR's encoder1 residual block (Cin = 1)
+  if (a.x_affine) return 0;            // neither special case has the per-channel input transform
   if (a.Cin == 1 && a.Cout <= 64 && (k133 || k333 || k111) && !a.x_stats && !a.act && !a.dbias) return 1;
   if (taps == 1 && a.Cout <= 16 && a.Cin <= 128 && a.Cin % 8 == 0 && a.x_ld % 8 == 0 && a.x_coff % 8 == 0 &&
       (reinterpret_cast<uintptr_t>(a.x) & 15) == 0) return 2;
@@ -445,7 +446,7 @@ pointwise_small_kernel(ConvArgs a) {
 
 int conv3d_fwd_small(const ConvArgs& a, int dtype, cudaStream_t st) {
   const int64_t V = (int64_t)a.D * a.H * a.W;
-  const bool plain = !a.x_stats && !a.act && !a.res && !a.gx;
+  const bool plain = !a.x_stats && !a.x_affine && !a.act && !a.res && !a.gx;
   const bool k133 = (a.kd == 1 && a.kh == 3 && a.kw == 3), k333 = (a.kd == 3 && a.kh == 3 && a.kw == 3);
   const bool k111s = (a.kd == 1 && a.kh == 1 && a.kw == 1);
   // stem_fwd_kernel stores y in 16-byte groups of 8 channels; pointwise_small_kernel moves x and y in 4-channel vectors

@@ -55,6 +55,7 @@ struct WgParams {
   alignas(64) CUtensorMap tm_dy;           // dy as {8 ch, w, h, plane, b*D+d}, box {8, TW, TS, min(Cout, MT)/8}
   alignas(64) CUtensorMap tm_x;            // x likewise, box {8, HALO_W, HALO_H, NTC/8}
   const double* x_stats; float eps; int act;   // x is normalised + activated in shared memory when x_stats / act
+  const float* x_affine; int per_channel;      // or transformed per channel (conv_args.h); the table is then [NTC]
   float* dw;
   float* part;                             // S > 1: split-K partials [S][Cout][Cin][taps], summed in split order
   int B, D, H, W, Cin, Cout, kd, kh, kw;
@@ -73,7 +74,7 @@ struct Bars {
   __device__ __forceinline__ uint32_t empty(int i) const { return bar0 + 8u * (uint32_t)(p.NS + i); }
   __device__ __forceinline__ uint32_t land(int i) const { return bar0 + 8u * (uint32_t)(2 * p.NS + i); }
   // what the consumers wait on: the transformed stage, or the raw stage straight off the TMA
-  __device__ __forceinline__ uint32_t ready(int i) const { return (p.x_stats || p.act) ? full(i) : land(i); }
+  __device__ __forceinline__ uint32_t ready(int i) const { return (p.x_stats || p.x_affine || p.act) ? full(i) : land(i); }
 };
 
 // blockIdx.x read afresh: a job decoded again after the register split, or after the MMA loop, is not merged with an
@@ -177,11 +178,12 @@ __device__ __forceinline__ void transform_role(const WgParams& p, const Job& job
     mbar_wait(bars.land(r.idx), r.phase);
     if (active) {
       uint8_t* sp = smem + r.idx * p.stage_bytes + p.dy_bytes + c8 * p.a_plane;
-      float sc[8], sf[8];                          // x*sc + sf == (x - mean) * rstd
+      float sc[8], sf[8];                          // x*sc + sf: (x - mean) * rstd, or the per-channel transform
+      const float2* tb = s_norm + (p.per_channel ? 0 : c.b * p.NTC) + c8 * 8;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const float2 mr = s_norm[c.b * p.NTC + c8 * 8 + j];
-        sc[j] = mr.y; sf[j] = -mr.x * mr.y;
+        const float2 st = tb[j];
+        sc[j] = st.x; sf[j] = st.y;
       }
       const int hb = c.h0(p) - ph, wb = c.w0() - pw;
       int hh = hh0, ww = ww0;
@@ -326,7 +328,7 @@ wgrad_tc_kernel(const __grid_constant__ WgParams p) {
   const int ci0 = decode_job(p, blockIdx.x).ci_tile * p.NTC;
 
   const Bars bars{smem_u32(smem + p.smem_bar_off), p};
-  float2* s_norm = reinterpret_cast<float2*>(smem + p.smem_norm_off);     // [B][NTC] {mean, rstd} of this job's channels
+  float2* s_norm = reinterpret_cast<float2*>(smem + p.smem_norm_off);     // [B or 1][NTC] {scale, shift} of this job's channels
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < p.NS; ++i) {
@@ -336,11 +338,15 @@ wgrad_tc_kernel(const __grid_constant__ WgParams p) {
   }
   {
     const double n = (double)p.D * p.H * p.W;
-    for (int i = threadIdx.x; i < p.B * p.NTC; i += kThreads) {
-      float m = 0.f, r = 1.f;
+    for (int i = threadIdx.x; i < (p.per_channel ? 1 : p.B) * p.NTC; i += kThreads) {
       const int b = i / p.NTC, c = i % p.NTC;
-      if (p.x_stats) stats_to_mean_rstd(p.x_stats + ((int64_t)b * p.Cin + ci0 + c) * 2, n, p.eps, m, r);
-      s_norm[i] = make_float2(m, r);
+      if (p.x_affine) {
+        s_norm[i] = make_float2(p.x_affine[2 * (ci0 + c)], p.x_affine[2 * (ci0 + c) + 1]);
+      } else {
+        float m = 0.f, r = 1.f;
+        if (p.x_stats) stats_to_mean_rstd(p.x_stats + ((int64_t)b * p.Cin + ci0 + c) * 2, n, p.eps, m, r);
+        s_norm[i] = make_float2(r, -m * r);
+      }
     }
   }
   __syncthreads();
@@ -352,7 +358,7 @@ wgrad_tc_kernel(const __grid_constant__ WgParams p) {
     const Job job = decode_job(p, cta_id());
     if (warp == kLoadWarp0) {
       if ((threadIdx.x & 31) == 0) tma_producer(p, job, smem, bars);
-    } else if (p.x_stats || p.act) {
+    } else if (p.x_stats || p.x_affine || p.act) {
       transform_role(p, job, smem, s_norm, bars);
     }
   } else {
@@ -393,7 +399,8 @@ bool fill_params(const WgradArgs& a, WgParams& p) {
   p.B = a.B; p.D = a.D; p.H = a.H; p.W = a.W; p.Cin = a.Cin; p.Cout = a.Cout; p.kd = a.kd; p.kh = a.kh; p.kw = a.kw;
   p.NTC = pick_ntc(a.Cin);
   if (!p.NTC || a.Cout % 8) return false;
-  if (a.B * p.NTC > 2048) return false;
+  const int nb = a.per_channel ? 1 : a.B;           // samples with their own row in the transform table
+  if (nb * p.NTC > 2048) return false;
   p.ci_tiles = a.Cin / p.NTC;
   p.co_tiles = (a.Cout + MT - 1) / MT;
   const int taps_hw = a.kh * a.kw;
@@ -405,7 +412,7 @@ bool fill_params(const WgradArgs& a, WgParams& p) {
   // whole planes, so with Cout not a multiple of 64 the last live warpgroup reads past them into the `a` tile, the
   // next stage or, from the last slot, the tail (rows computed from those values are never read back)
   const int co_max = a.Cout < MT ? a.Cout : MT;
-  const int norm_bytes = a.B * p.NTC * 8;
+  const int norm_bytes = nb * p.NTC * 8;
   int tail = 0;
   auto size_ring = [&](int ts) {
     p.TS = ts; p.halves = TH / ts;
@@ -472,9 +479,10 @@ int conv3d_wgrad_tc(const WgradArgs& a, int dtype, void* workspace, size_t ws_by
       !b200seg_make_act_tmap(&p.tm_x, a.x, a.x_ld, a.x_coff, a.Cin, a.B * a.D, a.H, a.W, p.HALO_W, p.HALO_H, p.NTC / 8))
     return B200SEG_ECUDA;
   p.x_stats = a.x_stats; p.eps = a.eps; p.act = a.act;
+  p.x_affine = a.x_affine; p.per_channel = a.per_channel;
   p.dw = a.dw;
   const int64_t jobs = (int64_t)p.co_tiles * p.ci_tiles * a.kd * p.ngroups;
-  const int smem_bytes = p.smem_norm_off + a.B * p.NTC * 8 + 64;
+  const int smem_bytes = p.smem_norm_off + (a.per_channel ? 1 : a.B) * p.NTC * 8 + 64;
   static thread_local bool attr_set = false;
   if (!attr_set) {
     B200_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));

@@ -42,5 +42,10 @@ def get_model(args, pretrain=False):
                          num_heads=12, pos_embed='perceptron', norm_name='instance', res_block=True)
         raise ValueError("model %r (3d) is not implemented by the H100 path" % (args.model,))
     if args.dimension == '2d':
-        raise ValueError("2d models are outside the GPU hot path (SURVEY.md §2); use the reference")
+        if args.model in ('unet', 'resunet'):
+            from .unet2d import UNet2D
+            if pretrain:
+                raise ValueError('No pretrain model available')   # model/utils.py:11-12
+            return UNet2D(args.in_chan, args.classes, args.base_chan, block=args.block)
+        raise ValueError("model %r (2d) is not implemented by the H100 path (2d: unet, resunet)" % (args.model,))
     raise ValueError("Invalid dimension, should be '2d' or '3d'")

@@ -1,5 +1,6 @@
 """Evaluation-side consumers of ``net(x)`` behind the reference's own function names (SURVEY.md §8f.2):
   inference_whole_image / inference_sliding_window / get_inference   inference/inference3d.py:8-92, inference/utils.py:1-40
+  inference_whole_image_2d / inference_sliding_window_2d            inference/inference2d.py (D = 1 on the same kernels)
   calculate_dice / calculate_dice_split                               metric/utils.py:33-82
   calculate_distance                                                  metric/utils.py:8-28
 Same signatures and return values (probabilities fp32 [B,classes,D,H,W]; (dice, intersection, summ) tensors); the
@@ -96,12 +97,55 @@ def inference_sliding_window(net, img, args, return_label=False):
     return (prob, label) if return_label else prob
 
 
+def _logits5(pred):
+    """[B,C,H,W] logits (any strides) as the [B,C,1,H,W] view the accumulation kernel takes."""
+    if isinstance(pred, (tuple, list)):
+        pred = pred[0]
+    return pred.unsqueeze(2)
+
+
+def inference_whole_image_2d(net, img, args=None):
+    """inference/inference2d.py inference_whole_image: img [B,C,H,W] (a slice stack) -> softmax [B,classes,H,W]."""
+    net.eval()
+    with torch.no_grad():
+        pred = _logits5(net(img))
+    _need_cuda(pred)
+    with on_device(pred):
+        B, C, _, H, W = pred.shape
+        prob = torch.zeros(B, C, 1, H, W, dtype=torch.float32, device=pred.device)
+        counter = torch.zeros(B, 1, 1, H, W, dtype=torch.float32, device=pred.device)
+        _softmax_accumulate(pred, prob, counter, (0, 0, 0, 1, H, W))
+    return prob[:, :, 0]
+
+
+def inference_sliding_window_2d(net, img, args):
+    """inference/inference2d.py inference_sliding_window: half-window stride, last window snapped to the border
+    (no padding: the image must be at least one window), softmax averaged over the windows; [B,classes,H,W]."""
+    net.eval()
+    _need_cuda(img)
+    B, C, H, W = img.shape
+    win_h, win_w = args.window_size
+    hh, hw = win_h // 2, win_w // 2
+    with on_device(img):
+        prob = torch.zeros(B, args.classes, 1, H, W, dtype=torch.float32, device=img.device)
+        counter = torch.zeros(B, 1, 1, H, W, dtype=torch.float32, device=img.device)
+        with torch.no_grad():
+            for i in range(H // hh):
+                for j in range(W // hw):
+                    h0, h1 = split_idx(hh, H, i)
+                    w0, w1 = split_idx(hw, W, j)
+                    pred = _logits5(net(img[:, :, h0:h1, w0:w1]))
+                    _softmax_accumulate(pred, prob, counter, (0, h0, w0, 1, h1 - h0, w1 - w0))
+        _lib.call("b200seg_normalize_argmax", prob.data_ptr(), counter.data_ptr(), None, B, args.classes, H * W, _stream())
+    return prob[:, :, 0]
+
+
 def get_inference(args):
-    """inference/utils.py:1-23 for the 3D path."""
+    """inference/utils.py:1-23."""
     if args.dimension == '3d':
         return inference_sliding_window if args.sliding_window else inference_whole_image
     if args.dimension == '2d':
-        raise ValueError("2d inference is outside the GPU hot path (SURVEY.md §2); use the reference")
+        return inference_sliding_window_2d if args.sliding_window else inference_whole_image_2d
     raise ValueError('Error in image dimension')
 
 

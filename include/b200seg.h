@@ -207,6 +207,67 @@ int b200seg_conv3d_wgrad(const void* x, int x_ld, int x_coff,
                          int kd, int kh, int kw, int dtype, int algo,
                          void* workspace, size_t ws_bytes, void* stream);
 
+/* ---- per-channel (BatchNorm) mode of the convolutions -------------------------
+ * The input enters as act(x[vox][c] * s[c] + t[c]) from x_affine, a float
+ * [Cin][2] {s, t} table (b200seg_batchnorm_fwd_fold), or as act(x) when
+ * x_affine is NULL.  The table is one row for the whole batch, so the algorithm
+ * and packed-weight layout of these launches are b200seg_conv3d_algo(..., B=1)
+ * at any B.  There is no data-gradient mask: the data gradient of a BatchNorm
+ * layer is a raw b200seg_conv3d_fwd_pc launch followed by
+ * b200seg_batchnorm_bwd_reduce / _fold / _apply.  Everything else (bias,
+ * residual, y_stats, workspace, accumulation into dw) is as in
+ * b200seg_conv3d_fwd / b200seg_conv3d_wgrad. */
+int b200seg_conv3d_fwd_pc(const void* x, int x_ld, int x_coff, const float* x_affine, int act,
+                          const void* w_packed, const float* bias,
+                          const void* residual, int r_ld, int r_coff,
+                          void* y, int y_ld, int y_coff, double* y_stats,
+                          int B, int D, int H, int W, int Cin, int Cout,
+                          int kd, int kh, int kw, int dtype, int algo, void* stream);
+size_t b200seg_conv3d_wgrad_pc_workspace(int x_ld, int x_coff, int transformed,
+                                         int dy_ld, int dy_coff, int want_bias,
+                                         int B, int D, int H, int W, int Cin, int Cout,
+                                         int kd, int kh, int kw, int dtype, int algo);
+int b200seg_conv3d_wgrad_pc(const void* x, int x_ld, int x_coff, const float* x_affine, int act,
+                            const void* dy, int dy_ld, int dy_coff,
+                            float* dw, float* dbias,
+                            int B, int D, int H, int W, int Cin, int Cout,
+                            int kd, int kh, int kw, int dtype, int algo,
+                            void* workspace, size_t ws_bytes, void* stream);
+
+/* ---- BatchNorm (nn.BatchNorm2d, training and eval) ------------------------------
+ * sums: fp64 [nb][C][2] {sum x, sum x^2} (nb = B for the per-(sample, channel) sums
+ * a convolution epilogue writes, 1 for sums already added over the batch or the
+ * ranks), count = values per channel.  Training: batch mean and biased variance;
+ * running_mean / running_var updated with `momentum` (running_var with the
+ * unbiased variance) and *num_batches_tracked += 1 (may be NULL); count <= 1 is
+ * B200SEG_EINVAL.  Eval: the running statistics.  Writes table [C][2] {s, t} =
+ * {gamma*rstd, beta - mean*gamma*rstd} and mean_rstd [C][2]. */
+int b200seg_batchnorm_fwd_fold(const double* sums, int nb, int C, double count,
+                               const float* gamma, const float* beta,
+                               float* running_mean, float* running_var, int64_t* num_batches_tracked,
+                               float momentum, float eps, int training,
+                               float* table, float* mean_rstd, void* stream);
+/* y = act(x*s + t) (post-activation blocks); C, ld and offsets multiples of 8. */
+int b200seg_batchnorm_apply(const void* x, int dtype, int x_ld, int x_coff, const float* table, int act,
+                            void* y, int y_ld, int y_coff, int64_t nvox, int C, void* stream);
+/* sums [C][2] (fp64, zeroed by the caller) += {sum dz, sum dz*xhat}, where
+ * dz = g * act'(x*s + t) (g itself when table is NULL or act is NONE) and
+ * xhat = (x - mean) * rstd.  C <= 2048. */
+int b200seg_batchnorm_bwd_reduce(const void* g, int g_ld, int g_coff, const void* x, int x_ld, int x_coff,
+                                 int dtype, const float* table, int act, const float* mean_rstd,
+                                 int64_t nvox, int C, double* sums, void* stream);
+/* dgamma = sum dz*xhat, dbeta = sum dz (fp32, written), and coef [C][4]
+ * {a, b, mean, k} with dx = a*dz + b*(x - mean) + k (training: batch-statistic
+ * terms included; eval: b = k = 0). */
+int b200seg_batchnorm_bwd_fold(const double* sums, double count, const float* gamma, const float* mean_rstd,
+                               int training, int C, float* dgamma, float* dbeta, float* coef, void* stream);
+/* out = a*dz + b*(x - mean) + k (+ add); dz as in b200seg_batchnorm_bwd_reduce.
+ * out may be add (accumulation in place). */
+int b200seg_batchnorm_bwd_apply(const void* g, int g_ld, int g_coff, const void* x, int x_ld, int x_coff,
+                                int dtype, const float* table, int act, const float* coef,
+                                const void* add, int add_ld, int add_coff,
+                                void* out, int out_ld, int out_coff, int64_t nvox, int C, void* stream);
+
 /* ---------------------------------------------------------------------------
  * MaxPool3d, kernel == stride (unet_utils.py:36), floor mode, + IN sums of the
  * pooled tensor.  idx: uint8[B][Do][Ho][Wo][C] argmax offset inside the window.
