@@ -88,6 +88,9 @@ _PROTOS = {
     "b200seg_aug_resample": [P, P, I, I, P, P, P, P, P, P, I, P, P, I, P, I, P],
     "b200seg_aug_pointwise": [P, P, I, L, I, P, P, P, P, P, ctypes.c_uint64, P],
     "b200seg_aug_gaussian_blur": [P, P, I, I, I, I, P, I, P, I, P],
+    "b200seg_aug_gaussian_blur2d": [P, P, I, I, I, P, I, P, I, P],
+    "b200seg_aug2d_workspace": [I, L],
+    "b200seg_aug2d_train": [P, I, L, I, I, I, P, P, P, ctypes.c_size_t, P],
     "b200seg_attn_gate_fwd": [P, I, P, P, I, I, F, P, P, P, I, I, P, I, L, I, I, I, P],
     "b200seg_attn_gate_bwd": [P, I, I, P, I, I, P, I, P, P, P, F, P, P, P, P, P, I, L, I, I, I, P],
     "b200seg_biattn_workspace": [I, L, I, I],
@@ -99,7 +102,7 @@ _RESTYPES = {"b200seg_strerror": c_char_p, "b200seg_last_cuda_error": c_char_p,
              "b200seg_conv3d_wgrad_workspace": ctypes.c_size_t, "b200seg_conv3d_wgrad_pc_workspace": ctypes.c_size_t, "b200seg_biattn_workspace": ctypes.c_size_t,
              "b200seg_mapgen_workspace": ctypes.c_size_t,
              "b200seg_channel_scale_bwd_workspace": ctypes.c_size_t, "b200seg_window_attn_workspace": ctypes.c_size_t,
-             "b200seg_surface_distance_workspace": ctypes.c_size_t}
+             "b200seg_surface_distance_workspace": ctypes.c_size_t, "b200seg_aug2d_workspace": ctypes.c_size_t}
 
 EXPORTED_SYMBOLS = tuple(_PROTOS)
 
@@ -138,7 +141,8 @@ def check(rc, what):
 
 # kernels launched per entry point (dice fwd = reduce + finalize; its memset is not ours)
 _KERNELS = {"b200seg_dice_ce_fwd": 2, "b200seg_biattn_fwd": 2, "b200seg_window_attn_bwd": 2, "b200seg_attention_bwd": 3, "b200seg_adamw_ema_step": 2, "b200seg_biattn_bwd": 2,
-            "b200seg_mapgen_fwd": 2, "b200seg_channel_scale_bwd_reduce": 2, "b200seg_attn_gate_fwd": 2, "b200seg_attn_gate_bwd": 2}
+            "b200seg_mapgen_fwd": 2, "b200seg_channel_scale_bwd_reduce": 2, "b200seg_attn_gate_fwd": 2, "b200seg_attn_gate_bwd": 2,
+            "b200seg_aug2d_train": 3}
 launch_count = 0
 
 

@@ -10,15 +10,20 @@ per intensity op, a dense 5^3/7^3 ``F.conv3d`` blur and a host-generated noise v
     ``csrc/augment.cu`` instead of library calls;
   * :class:`TrainAugment3D` is the whole training branch as a *plan + 2..7 launches*: all random numbers are drawn first
     (they never depend on data), then ONE gather produces the final patch (crop -> affine -> centre crop -> mirrors), and
-    each intensity op reads the statistics its predecessor left on the device — no reduction passes, no host sync.
+    each intensity op reads the statistics its predecessor left on the device — no reduction passes, no host sync;
+  * :class:`TrainAugment2D` is the 2D (ACDC) slice branch for a whole batch of ragged slices in three launches
+    (``b200seg_aug2d_train``), writing the ``[B, 1, h, w]`` batch the 2D models and losses take.
 
-Images are ``[1, C, D, H, W]`` fp32 CUDA tensors, label maps ``[1, 1, D, H, W]`` uint8 or int64.  There is no CPU path."""
+Images are ``[1, C, D, H, W]`` (volumes) or ``[1, C, H, W]`` (slices) fp32 CUDA tensors, label maps ``[1, 1, D, H, W]``
+or ``[1, 1, H, W]`` uint8 or int64.  The 2D geometry runs on the 3D gather with D = 1.  There is no CPU path."""
 import math
+import struct
 
 import numpy as np
 import torch
 
 from ._lib import B200SegError, call
+from ._lib import load as load_lib
 from .ops import _need_cuda, _stream
 
 OP_MUL, OP_ADD, OP_GAMMA_POW, OP_RENORM, OP_CONTRAST, OP_NOISE, OP_STATS = range(7)
@@ -54,11 +59,19 @@ def decode_stats(stats, n):
 
 def _img(t):
     _need_cuda(t)
-    if t.dim() != 5 or t.shape[0] != 1:
-        raise ValueError("expected a [1, C, D, H, W] volume (2D augmentation is outside the GPU hot path)")
+    if t.dim() not in (4, 5) or t.shape[0] != 1:
+        raise ValueError("expected a [1, C, D, H, W] volume or a [1, C, H, W] image")
     if t.dtype != torch.float32:
         raise TypeError("images are fp32 (the reference augments before autocast), got %s" % t.dtype)
     return t.contiguous()
+
+
+def _vol(*ts):
+    """The volume functions take [1, C, D, H, W] tensors only: a [1, C, H, W] slice would hand the gather two-element
+    geometry arrays where it reads three (the 2D functions make the [1, C, 1, H, W] view themselves)."""
+    for t in ts:
+        if t is not None and t.dim() != 5:
+            raise ValueError("expected a [1, C, D, H, W] volume, got %s (use the 2D functions for slices)" % list(t.shape))
 
 
 def _lab(t):
@@ -100,6 +113,9 @@ def image_stats(tensor_img, per_channel=False):
 def resample(tensor_img, tensor_lab, sub_origin, sub_size, theta, out_origin, out_size, flips=(False, False, False),
              want_stats=False, per_channel=False, out_label_dtype=torch.int64):
     """The fused gather (``b200seg_aug_resample``).  theta: [3,4] float tensor / array (affine branch) or None (copy)."""
+    _vol(tensor_img, tensor_lab)
+    if any(len(v) != 3 for v in (sub_origin, sub_size, out_origin, out_size, flips)):
+        raise ValueError("origins, sizes and flips of the volume gather have three entries (D, H, W)")
     img = None if tensor_img is None else _img(tensor_img)
     lab = None if tensor_lab is None else _lab(tensor_lab)
     ref = img if img is not None else lab
@@ -150,8 +166,66 @@ def draw_affine_theta(scale=0.3, rotate=45, translate=0.1, shear=0.05):
     return theta[0:3, :].contiguous()
 
 
+def draw_affine_theta_2d(scale=0.3, rotate=180, translate=0):
+    """The random 2x3 matrix of ``random_scale_rotate_translate_2d`` (augmentation.py:192-214): six np.random.random()
+    draws (x/y scale, x/y shear, x/y translation), then one integer angle; fp32 product S @ R."""
+    scale = [scale] * 2 if isinstance(scale, (int, float)) else list(scale)
+    translate = [translate] * 2 if isinstance(translate, (int, float)) else list(translate)
+    sx = 1 - scale[0] + np.random.random() * 2 * scale[0]
+    sy = 1 - scale[1] + np.random.random() * 2 * scale[1]
+    hx = np.random.random() * 2 * scale[0] - scale[0]
+    hy = np.random.random() * 2 * scale[1] - scale[1]
+    tx = np.random.random() * 2 * translate[0] - translate[0]
+    ty = np.random.random() * 2 * translate[1] - translate[1]
+    S = torch.tensor([[sx, hx, tx], [hy, sy, ty], [0, 0, 1]]).float()
+    a = (float(np.random.randint(-rotate, max(rotate, 1))) / 180.) * math.pi
+    R = torch.tensor([[math.cos(a), -math.sin(a), 0], [math.sin(a), math.cos(a), 0], [0, 0, 1]]).float()
+    return torch.mm(S, R)[0:2, :].contiguous()
+
+
+def embed_theta_2d(theta):
+    """A 2x3 theta as the 3x4 of the volume gather on a D = 1 grid: the z tap weight is exactly 0, so trilinear
+    sampling of the one plane is bilinear sampling."""
+    t = torch.as_tensor(theta, dtype=torch.float32).reshape(2, 3)
+    out = torch.zeros(3, 4)
+    out[:2, :2], out[:2, 3], out[2, 2] = t[:, :2], t[:, 2], 1.0
+    return out
+
+
+def _as_volume(t):
+    """[1, C, H, W] -> the [1, C, 1, H, W] view the volume kernels take."""
+    return None if t is None else t.unsqueeze(2)
+
+
+def random_scale_rotate_translate_2d(tensor_img, tensor_lab, scale, rotate, translate):
+    """augmentation.py:192-223 on the whole slice."""
+    theta = embed_theta_2d(draw_affine_theta_2d(scale, rotate, translate))
+    size = [1] + list(tensor_img.shape[2:])
+    img, lab, _ = resample(_as_volume(tensor_img), _as_volume(tensor_lab), (0, 0, 0), size, theta, (0, 0, 0), size)
+    return img.squeeze(2), lab.squeeze(2)
+
+
+def crop_2d(tensor_img, tensor_lab, crop_size, mode):
+    """augmentation.py:297-317 (slicing clamps at the slice border, as Python slices do)."""
+    assert mode in ['random', 'center'], "Invalid Mode, should be 'random' or 'center'"
+    crop_size = [crop_size] * 2 if isinstance(crop_size, int) else list(crop_size)
+    shape = list(tensor_img.shape[2:])
+    if mode == 'random':
+        org = _crop_origin_random(shape, crop_size)
+    else:
+        org = [(s - c) // 2 for s, c in zip(shape, crop_size)]
+    if min(org) < 0:
+        raise ValueError("centre crop larger than the slice (the reference's negative slice start is not supported)")
+    size = [min(c, s - o) for c, s, o in zip(crop_size, shape, org)]
+    lab = _lab(tensor_lab)
+    img, olab, _ = resample(_as_volume(tensor_img), _as_volume(lab), [0] + org, [1] + size, None, (0, 0, 0), [1] + size,
+                            out_label_dtype=lab.dtype)
+    return img.squeeze(2), olab.squeeze(2)
+
+
 def random_scale_rotate_translate_3d(tensor_img, tensor_lab, scale=0.3, rotate=45, translate=0.1, shear=0.05):
     """augmentation.py:226-291 on the whole input volume."""
+    _vol(tensor_img, tensor_lab)
     theta = draw_affine_theta(scale, rotate, translate, shear)
     size = list(tensor_img.shape[2:])
     img, lab, _ = resample(tensor_img, tensor_lab, (0, 0, 0), size, theta, (0, 0, 0), size)
@@ -166,6 +240,7 @@ def _crop_origin_random(shape, crop_size):
 def crop_3d(tensor_img, tensor_lab, crop_size, mode):
     """augmentation.py:320-343 (slicing clamps at the volume border, as Python slices do)."""
     assert mode in ['random', 'center'], "Invalid Mode, should be 'random' or 'center'"
+    _vol(tensor_img, tensor_lab)
     crop_size = _triple(crop_size) if isinstance(crop_size, int) else list(crop_size)
     shape = list(tensor_img.shape[2:])
     if mode == 'random':
@@ -182,6 +257,7 @@ def crop_3d(tensor_img, tensor_lab, crop_size, mode):
 def crop_around_coordinate_3d(tensor_img, tensor_lab, crop_size, coordinate, mode):
     """augmentation.py:346-383."""
     assert mode in ['random', 'center'], "Invalid Mode, should be 'random' or 'center'"
+    _vol(tensor_img, tensor_lab)
     crop_size = _triple(crop_size) if isinstance(crop_size, int) else list(crop_size)
     shape = list(tensor_img.shape[2:])
     org = []
@@ -197,8 +273,12 @@ def crop_around_coordinate_3d(tensor_img, tensor_lab, crop_size, coordinate, mod
 
 
 def mirror(tensor_img, axis=0):
-    """torch.flip(dims=[2+axis]) (augmentation.py:176-197) for an image or a label map."""
+    """torch.flip(dims=[2+axis]) (augmentation.py:176-197) for an image or a label map, volume or slice."""
+    if tensor_img.dim() == 4:
+        assert axis in [0, 1], "axis should be either 0 or 1 for 2D images"
+        return mirror(_as_volume(tensor_img), axis + 1).squeeze(2)
     assert axis in [0, 1, 2], "axis should be either 0, 1 or 2 for volume images"
+    _vol(tensor_img)
     flips = [axis == 0, axis == 1, axis == 2]
     size = list(tensor_img.shape[2:])
     if tensor_img.dtype == torch.float32:
@@ -216,7 +296,8 @@ def gaussian_noise(tensor_img, std, mean=0):
 
 
 def gaussian_kernel_1d(kernel_size, sigma):
-    """1-D factor of generate_3d_gaussian_kernel (augmentation.py:31-44): the normalised dense kernel is its outer cube."""
+    """1-D factor of generate_3d_gaussian_kernel / generate_2d_gaussian_kernel (augmentation.py:18-44): the normalised
+    dense kernel is its outer cube / outer square."""
     r = torch.arange(-kernel_size // 2 + 1, kernel_size // 2 + 1, dtype=torch.float32)
     w = torch.exp(-(r ** 2) / (2 * float(sigma) ** 2))
     return (w / w.sum()).contiguous()
@@ -229,6 +310,11 @@ def _blur(tensor_img, sigma, want_stats=False, per_channel=False):
     y = torch.empty_like(x)
     rows = _rows(x.shape[1], per_channel)
     so = new_stats(rows, x.device) if want_stats else None
+    if x.dim() == 4:
+        _, C, H, W = x.shape
+        call("b200seg_aug_gaussian_blur2d", x.data_ptr(), y.data_ptr(), C, H, W, w.data_ptr(), kernel_size,
+             None if so is None else so.data_ptr(), rows, _stream())
+        return y, so
     _, C, D, H, W = x.shape
     call("b200seg_aug_gaussian_blur", x.data_ptr(), y.data_ptr(), C, D, H, W, w.data_ptr(), kernel_size,
          None if so is None else so.data_ptr(), rows, _stream())
@@ -244,7 +330,7 @@ def gaussian_blur(tensor_img, sigma_range=[0.5, 1.0]):
 def brightness_additive(tensor_img, std, mean=0, per_channel=False):
     """augmentation.py:66-85."""
     C = tensor_img.shape[1] if per_channel else 1
-    r = torch.normal(mean, std, size=(1, C, 1, 1, 1))
+    r = torch.normal(mean, std, size=(1, C) + (1,) * (tensor_img.dim() - 2))
     return _pointwise(tensor_img, OP_ADD, a=r, rows=C)[0]
 
 
@@ -252,7 +338,7 @@ def brightness_multiply(tensor_img, multiply_range=[0.7, 1.3], per_channel=False
     """augmentation.py:88-101."""
     assert multiply_range[1] > multiply_range[0], 'Invalid range'
     C = tensor_img.shape[1] if per_channel else 1
-    r = torch.rand(size=(1, C, 1, 1, 1)) * (multiply_range[1] - multiply_range[0]) + multiply_range[0]
+    r = torch.rand(size=(1, C) + (1,) * (tensor_img.dim() - 2)) * (multiply_range[1] - multiply_range[0]) + multiply_range[0]
     return _pointwise(tensor_img, OP_MUL, a=r, rows=C)[0]
 
 
@@ -340,6 +426,7 @@ class TrainAugment3D:
         return p
 
     def apply(self, tensor_img, tensor_lab, p):
+        _vol(tensor_img, tensor_lab)
         C = tensor_img.shape[1]
         need_stats = p["gamma"] is not None or p["contrast"] is not None
         img, lab, st = resample(tensor_img, tensor_lab, p["sub_origin"], p["sub_size"], p["theta"], p["out_origin"],
@@ -359,6 +446,120 @@ class TrainAugment3D:
         return img, lab
 
     def __call__(self, tensor_img, tensor_lab):
+        _vol(tensor_img, tensor_lab)                      # before any draw
         if not tensor_img.is_cuda:
             raise B200SegError("b200seg.augmentation runs on an H100 only — there is no CPU fallback")
         return self.apply(tensor_img, tensor_lab, self.plan(tensor_img.shape[2:], tensor_img.shape[1]))
+
+
+# ----------------------------------------------------------------------------- the 2D slice branch for a whole batch
+_ROW = struct.Struct("<QQQiiQfff6fiii")          # b200seg_aug2d_row (include/b200seg.h), 88 bytes
+assert _ROW.size == 88
+
+
+class TrainAugment2D:
+    """The ``mode == 'train'`` branch of the 2D ACDC dataset's ``__getitem__`` (dataset_acdc.py:128-142), for a batch
+    of B slices of their own H x W: gaussian_noise -> brightness_additive -> gamma(retain_stats) ->
+    random_scale_rotate_translate_2d -> crop_2d(random), every op applied (no coin flips in that branch).
+
+    ``plan()`` makes one slice's draws in the order of the public functions above (noise key, brightness, gamma, the six
+    affine numbers and the angle, the two crop offsets).  The numpy draws, and so the geometry and the crop, are the
+    reference's for the same ``np.random`` state.  The torch draws are not: the reference's ``torch.randn`` of the
+    whole slice consumes as many numbers as the slice has pixels, where the noise here is a counter-based Philox
+    stream keyed by one ``torch.randint`` draw (the key :func:`gaussian_noise` uses).
+
+    ``apply()`` runs the plans as one batch in three launches (``b200seg_aug2d_train``): two per-slice statistics
+    passes and one gather of the h x w crops.  It returns ``img [B, 1, h, w]`` fp32 and ``lab [B, 1, h, w]`` int64,
+    the layout ``UNet2D`` and ``DiceCELoss`` take.  The slice statistics never leave the device, and a given plan gives
+    the same bits on every run."""
+
+    def __init__(self, training_size, scale=0.3, rotate=180, translate=0, gaussian_noise_std=0.02,
+                 additive_brightness_std=0.7, gamma_range=(0.5, 1.6)):
+        self.size = [training_size] * 2 if isinstance(training_size, int) else list(training_size)
+        self.scale, self.rotate, self.translate = scale, rotate, translate
+        self.noise_std, self.brightness_std, self.gamma_range = float(gaussian_noise_std), additive_brightness_std, gamma_range
+
+    def plan(self, slice_shape):
+        H, W = [int(s) for s in slice_shape[-2:]]
+        h, w = self.size
+        if H < h or W < w:
+            raise ValueError("slice %dx%d is smaller than the training size %dx%d" % (H, W, h, w))
+        p = {"noise_std": self.noise_std}
+        p["noise_key"] = int(torch.randint(0, 2 ** 62, (1,)).item())
+        p["beta"] = float(torch.normal(0, self.brightness_std, size=(1, 1, 1, 1)))
+        p["gamma"] = float(torch.rand(1, 1) * (self.gamma_range[1] - self.gamma_range[0]) + self.gamma_range[0])
+        p["theta"] = draw_affine_theta_2d(self.scale, self.rotate, self.translate)
+        p["crop"] = _crop_origin_random([H, W], self.size)
+        return p
+
+    @staticmethod
+    def _slice(t, what):
+        _need_cuda(t)
+        if t.dim() == 4:
+            if t.shape[0] != 1 or t.shape[1] != 1:
+                raise ValueError("%s must be [H, W] or [1, 1, H, W] (one channel), got %s" % (what, list(t.shape)))
+            t = t[0, 0]
+        elif t.dim() != 2:
+            raise ValueError("%s must be [H, W] or [1, 1, H, W], got %s" % (what, list(t.shape)))
+        return t.contiguous()
+
+    def apply(self, images, labels, plans, y1_out=None):
+        """y1_out (optional, for tests): a list of contiguous fp32 [H, W] tensors on the images' device, one per slice,
+        that receive each slice's noisy, brightened image y1 = x + std * n + beta."""
+        return self._prepare(images, labels, plans, y1_out)()
+
+    def _prepare(self, images, labels, plans, y1_out=None):
+        """Check the inputs, pack and upload the table, allocate the outputs; returns a function that launches the
+        batch (``b200seg_aug2d_train``) and returns (img, lab)."""
+        if not (len(images) == len(labels) == len(plans)) or not images:
+            raise ValueError("images, labels and plans must be non-empty lists of the same length")
+        imgs = [self._slice(t, "image") for t in images]
+        labs = [self._slice(t, "label map") for t in labels]
+        for x, l in zip(imgs, labs):
+            if x.dtype != torch.float32:
+                raise TypeError("images are fp32 (the reference augments before autocast), got %s" % x.dtype)
+            if x.shape != l.shape:
+                raise ValueError("image %s and label map %s differ in shape" % (list(x.shape), list(l.shape)))
+            if x.shape[0] < self.size[0] or x.shape[1] < self.size[1]:
+                raise ValueError("slice %s is smaller than the training size %s" % (list(x.shape), self.size))
+        if y1_out is not None:
+            if len(y1_out) != len(imgs):
+                raise ValueError("y1_out needs one tensor per slice")
+            for x, y in zip(imgs, y1_out):
+                _need_cuda(y)
+                if y.device != x.device or y.dtype != torch.float32 or y.shape != x.shape or not y.is_contiguous():
+                    raise ValueError("y1_out tensors are contiguous fp32 [H, W] on the images' device, one per slice; got "
+                                     "%s %s %s for a %s slice" % (y.dtype, list(y.shape), y.device, list(x.shape)))
+        lab_dt = torch.uint8 if all(l.dtype == torch.uint8 for l in labs) else torch.int64
+        labs = [l.to(lab_dt) for l in labs]
+        h, w = self.size
+        B, dev = len(imgs), imgs[0].device
+        table = bytearray()
+        for i, (x, l, p) in enumerate(zip(imgs, labs, plans)):
+            oy, ox = p["crop"]
+            if not (0 <= oy <= x.shape[0] - h and 0 <= ox <= x.shape[1] - w):
+                raise ValueError("crop origin %s outside slice %s" % ((oy, ox), list(x.shape)))
+            y1 = 0 if y1_out is None else y1_out[i].data_ptr()
+            th = torch.as_tensor(p["theta"], dtype=torch.float32).reshape(6).tolist()
+            table += _ROW.pack(x.data_ptr(), l.data_ptr(), y1, x.shape[0], x.shape[1], p["noise_key"] & 0xFFFFFFFFFFFFFFFF,
+                               p["noise_std"], p["beta"], p["gamma"], *th, oy, ox, 0)
+        rows = torch.frombuffer(table, dtype=torch.uint8)
+        if dev.type == "cuda":
+            rows = rows.pin_memory()
+        rows = rows.to(dev, non_blocking=True)          # the one host-to-device copy of the call
+        max_elems = max(x.numel() for x in imgs)
+        ws_bytes = int(load_lib().b200seg_aug2d_workspace(B, max_elems))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        out_img = torch.empty(B, 1, h, w, dtype=torch.float32, device=dev)
+        out_lab = torch.empty(B, 1, h, w, dtype=torch.int64, device=dev)
+
+        def launch():
+            call("b200seg_aug2d_train", rows.data_ptr(), B, max_elems, labs[0].element_size(), h, w, out_img.data_ptr(),
+                 out_lab.data_ptr(), ws.data_ptr(), ws_bytes, _stream())
+            return out_img, out_lab
+        launch.inputs = imgs          # the (possibly copied) slices the table points at live as long as the launcher
+        return launch
+
+    def __call__(self, images, labels):
+        imgs = [self._slice(t, "image") for t in images]       # shapes and devices are checked before any draw
+        return self.apply(imgs, labels, [self.plan(t.shape) for t in imgs])

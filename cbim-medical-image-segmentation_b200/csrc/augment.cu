@@ -228,14 +228,19 @@ __global__ void __launch_bounds__(256) aug_pointwise_kernel(const float* __restr
 constexpr int BT_Z = 8, BT_Y = 8, BT_X = 32, BR_MAX = 3;      // output tile, maximum radius (k = 7)
 struct BlurW { float w[2 * BR_MAX + 1]; };
 
+// DEPTH = false is the 2-D blur of a [C][1][H][W] image (F.conv2d with the k x k kernel): tiles one plane deep and
+// no z pass, since the normalised 2-D kernel is the outer product of the two normalised 1-D ones.
+template <bool DEPTH>
 __global__ void __launch_bounds__(256) aug_blur_kernel(const float* __restrict__ x, float* __restrict__ y, int C, int D, int H, int W, int R,
                                                        BlurW kw, StatRow* __restrict__ sout, int stats_rows) {
   extern __shared__ float sm[];
-  const int EZ = BT_Z + 2 * R, EY = BT_Y + 2 * R, EX = BT_X + 2 * R;
+  constexpr int TZ = DEPTH ? BT_Z : 1;
+  const int RZ = DEPTH ? R : 0;
+  const int EZ = TZ + 2 * RZ, EY = BT_Y + 2 * R, EX = BT_X + 2 * R;
   float* s_in = sm;                          // [EZ][EY][EX]
   float* s_x = sm + EZ * EY * EX;            // [EZ][EY][BT_X]   after the x pass
   float* s_y = s_x + EZ * EY * BT_X;         // [EZ][BT_Y][BT_X] after the y pass
-  const int tx = (W + BT_X - 1) / BT_X, ty = (H + BT_Y - 1) / BT_Y, tz = (D + BT_Z - 1) / BT_Z;
+  const int tx = (W + BT_X - 1) / BT_X, ty = (H + BT_Y - 1) / BT_Y, tz = (D + TZ - 1) / TZ;
   const int64_t tiles = (int64_t)C * tz * ty * tx, V = (int64_t)D * H * W;
   float mn = INFINITY, mx = -INFINITY; double ssum = 0.0, ssq = 0.0;
   int cur_c = -1;
@@ -248,7 +253,7 @@ __global__ void __launch_bounds__(256) aug_blur_kernel(const float* __restrict__
     }
     cur_c = c;
     const float* xc = x + c * V;
-    const int z0 = bz * BT_Z - R, y0 = by * BT_Y - R, x0 = bx * BT_X - R;
+    const int z0 = bz * TZ - RZ, y0 = by * BT_Y - R, x0 = bx * BT_X - R;
     for (int i = threadIdx.x; i < EZ * EY * EX; i += 256) {
       const int lx = i % EX, ly = (i / EX) % EY, lz = i / (EX * EY);
       const int gz = z0 + lz, gy = y0 + ly, gx = x0 + lx;
@@ -273,13 +278,14 @@ __global__ void __launch_bounds__(256) aug_blur_kernel(const float* __restrict__
       s_y[i] = a;
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < BT_Z * BT_Y * BT_X; i += 256) {
+    for (int i = threadIdx.x; i < TZ * BT_Y * BT_X; i += 256) {
       const int lx = i % BT_X, ly = (i / BT_X) % BT_Y, lz = i / (BT_X * BT_Y);
-      const int gz = bz * BT_Z + lz, gy = by * BT_Y + ly, gx = bx * BT_X + lx;
+      const int gz = bz * TZ + lz, gy = by * BT_Y + ly, gx = bx * BT_X + lx;
       if (gz < D && gy < H && gx < W) {
         const float* p = s_y + (lz * BT_Y + ly) * BT_X + lx;
         float a = 0.f;
-        for (int k = 0; k <= 2 * R; ++k) a = fmaf(p[k * BT_Y * BT_X], kw.w[k], a);
+        if (DEPTH) { for (int k = 0; k <= 2 * R; ++k) a = fmaf(p[k * BT_Y * BT_X], kw.w[k], a); }
+        else a = p[0];
         y[c * V + ((int64_t)gz * H + gy) * W + gx] = a;
         mn = fminf(mn, a); mx = fmaxf(mx, a); ssum += a; ssq += (double)a * a;
       }
@@ -290,6 +296,205 @@ __global__ void __launch_bounds__(256) aug_blur_kernel(const float* __restrict__
     // every block owns tiles of increasing channel index; with one row, or the last channel of several, commit what is left
     if (stats_rows > 1) { if (cur_c >= 0) block_stats_commit(mn, mx, ssum, ssq, sout + cur_c); }
     else block_stats_commit(mn, mx, ssum, ssq, sout);
+  }
+}
+
+// ---- the batched 2-D training branch (training/dataset/dim2/dataset_acdc.py:128-142) ------------------------------
+// gaussian_noise -> brightness_additive -> gamma(retain_stats) -> random_scale_rotate_translate_2d -> crop_2d(random)
+// for B ragged slices in three launches.  y1 = x + std*n + beta is recomputed from x wherever it is needed (the noise
+// is counter-based), so no intermediate slice exists in HBM:
+//   aug2d_stats1: per-chunk {min, max, sum, sumsq} of y1;
+//   aug2d_stats2: per-chunk {sum, sumsq} of y2 = ((y1 - min)/rng)^gamma * rng + min;
+//   aug2d_gather: for each pixel of the h x w crop, the bilinear / nearest taps of the affine grid over the whole slice,
+//                 each tap's y3 = (y2 - mean2)/std2 * std1 + mean1 recomputed from x.
+// Every slice is cut into chunks of AUG2D_CHUNK elements; each block reduces its chunk in a fixed tree and writes one
+// partial, and the next launch folds a slice's partials in a fixed order (no atomics), so a plan always gives the same
+// bits, whatever the batch it runs in.
+constexpr int AUG2D_THREADS = 256, AUG2D_GROUPS = 4, AUG2D_CHUNK = AUG2D_THREADS * AUG2D_GROUPS * 4;
+static_assert(sizeof(b200seg_aug2d_row) == 88, "b200seg_aug2d_row layout is part of the ABI");
+
+struct Aug2dPart { double s, q; float mn, mx; float pad[2]; };
+
+__device__ __forceinline__ int aug2d_chunks(int64_t n) { return (int)((n + AUG2D_CHUNK - 1) / AUG2D_CHUNK); }
+
+// y1 with the exact expressions of OP_NOISE (mean 0) and OP_ADD, so the chain of per-function calls gives the same bits
+__device__ __forceinline__ float aug2d_y1(float x, float z, float std, float beta) {
+  const float zero = 0.f;
+  float v = x + z * std + zero;
+  return v + beta;
+}
+
+// the normal of element idx (component idx % 4 of Philox block idx / 4), as aug_pointwise_kernel<OP_NOISE> draws it
+__device__ __forceinline__ float aug2d_normal(uint64_t key, int64_t idx) {
+  float z[4];
+  philox_normal4(key, (uint64_t)(idx >> 2), z);
+  const int k = (int)(idx & 3);
+  return k == 0 ? z[0] : (k == 1 ? z[1] : (k == 2 ? z[2] : z[3]));
+}
+
+// block-wide fixed-order merge (256 threads) -> thread 0 holds the result
+__device__ __forceinline__ void aug2d_block_merge(float& mn, float& mx, double& s, double& q) {
+  __shared__ float s_mn[AUG2D_THREADS / 32], s_mx[AUG2D_THREADS / 32];
+  __shared__ double s_s[AUG2D_THREADS / 32], s_q[AUG2D_THREADS / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
+  s = warp_sum_d(s); q = warp_sum_d(q);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) { s_mn[w] = mn; s_mx[w] = mx; s_s[w] = s; s_q[w] = q; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 1; i < AUG2D_THREADS / 32; ++i) { mn = fminf(mn, s_mn[i]); mx = fmaxf(mx, s_mx[i]); s += s_s[i]; q += s_q[i]; }
+  }
+}
+
+// fold a slice's partials in a fixed order (warp 0: lane-strided serial sums, then a fixed xor tree); every lane of
+// warp 0 ends with the same values
+__device__ __forceinline__ void aug2d_fold(const Aug2dPart* p, int n, float& mn, float& mx, double& s, double& q) {
+  mn = INFINITY; mx = -INFINITY; s = 0.0; q = 0.0;
+  for (int i = threadIdx.x; i < n; i += 32) { const Aug2dPart a = p[i]; mn = fminf(mn, a.mn); mx = fmaxf(mx, a.mx); s += a.s; q += a.q; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
+  s = warp_sum_d(s); q = warp_sum_d(q);
+}
+
+// mean and unbiased std as read_stats computes them from the sums
+__device__ __forceinline__ void aug2d_moments(double s, double q, double n, double& mean, double& std) {
+  mean = s / n;
+  const double var = (q - n * mean * mean) / (n > 1.0 ? n - 1.0 : 1.0);
+  std = sqrt(var > 0.0 ? var : 0.0);
+}
+
+// the per-slice constants of the intensity chain, folded from the partials by warp 0 and broadcast through shared memory
+struct Aug2dConsts { float mn1, rng1, mean2, std2, std1, mean1; };
+
+template <bool SECOND>
+__device__ __forceinline__ void aug2d_consts(const Aug2dPart* p1, const Aug2dPart* p2, int nch, double n, Aug2dConsts& out) {
+  __shared__ Aug2dConsts sc;
+  if (threadIdx.x < 32) {
+    float mn, mx; double s, q;
+    aug2d_fold(p1, nch, mn, mx, s, q);
+    double m1, sd1; aug2d_moments(s, q, n, m1, sd1);
+    Aug2dConsts c = {mn, mx - mn, 0.f, 0.f, (float)sd1, (float)m1};
+    if (SECOND) {
+      aug2d_fold(p2, nch, mn, mx, s, q);
+      double m2, sd2; aug2d_moments(s, q, n, m2, sd2);
+      c.mean2 = (float)m2; c.std2 = (float)sd2;
+    }
+    if (threadIdx.x == 0) sc = c;
+  }
+  __syncthreads();
+  out = sc;
+}
+
+// PASS 1: partials of y1 (and, when the row asks for it, y1 itself); PASS 2: partials of y2
+template <int PASS>
+__global__ void __launch_bounds__(AUG2D_THREADS) aug2d_stats_kernel(const b200seg_aug2d_row* __restrict__ rows, int max_chunks,
+                                                                   Aug2dPart* __restrict__ part1, Aug2dPart* __restrict__ part2) {
+  const int b = blockIdx.y, c = blockIdx.x;
+  const b200seg_aug2d_row r = rows[b];
+  const int64_t n = (int64_t)r.H * r.W;
+  const int nch = aug2d_chunks(n);
+  if (c >= nch || nch > max_chunks) return;
+  Aug2dConsts k = {};
+  if (PASS == 2) aug2d_consts<false>(part1 + (int64_t)b * max_chunks, nullptr, nch, (double)n, k);
+  const float* x = r.img;
+  float* y1out = PASS == 1 ? r.y1 : nullptr;
+  const bool vec = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y1out)) & 15) == 0;
+  float mn = INFINITY, mx = -INFINITY; double sm = 0.0, sq = 0.0;
+#pragma unroll
+  for (int gi = 0; gi < AUG2D_GROUPS; ++gi) {
+    const int64_t g = (int64_t)c * (AUG2D_CHUNK / 4) + gi * AUG2D_THREADS + threadIdx.x;
+    const int64_t i0 = g * 4;
+    if (i0 >= n) break;
+    const int cnt = (int)((n - i0) < 4 ? (n - i0) : 4);
+    float v[4] = {0.f, 0.f, 0.f, 0.f}, z[4] = {0.f, 0.f, 0.f, 0.f};
+    if (vec && cnt == 4) { const float4 f = *reinterpret_cast<const float4*>(x + i0); v[0] = f.x; v[1] = f.y; v[2] = f.z; v[3] = f.w; }
+    else {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) if (e < cnt) v[e] = x[i0 + e];
+    }
+    if (r.noise_std != 0.f) philox_normal4(r.noise_key, (uint64_t)g, z);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      v[e] = aug2d_y1(v[e], z[e], r.noise_std, r.beta);
+      if (PASS == 2) v[e] = powf((v[e] - k.mn1) / k.rng1, r.gamma) * k.rng1 + k.mn1;
+      if (e < cnt) { mn = fminf(mn, v[e]); mx = fmaxf(mx, v[e]); sm += v[e]; sq += (double)v[e] * v[e]; }
+    }
+    if (y1out) {
+      if (vec && cnt == 4) *reinterpret_cast<float4*>(y1out + i0) = make_float4(v[0], v[1], v[2], v[3]);
+      else {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) if (e < cnt) y1out[i0 + e] = v[e];
+      }
+    }
+  }
+  aug2d_block_merge(mn, mx, sm, sq);
+  if (threadIdx.x == 0) {
+    Aug2dPart o = {sm, sq, mn, mx, {0.f, 0.f}};
+    (PASS == 1 ? part1 : part2)[(int64_t)b * max_chunks + c] = o;
+  }
+}
+
+// y3 of element idx of slice r
+__device__ __forceinline__ float aug2d_y3(const b200seg_aug2d_row& r, int64_t idx, const Aug2dConsts& k) {
+  const float z = r.noise_std != 0.f ? aug2d_normal(r.noise_key, idx) : 0.f;
+  const float y1 = aug2d_y1(r.img[idx], z, r.noise_std, r.beta);
+  const float y2 = powf((y1 - k.mn1) / k.rng1, r.gamma) * k.rng1 + k.mn1;
+  return (y2 - k.mean2) / k.std2 * k.std1 + k.mean1;
+}
+
+// one thread = one pixel of slice blockIdx.y's h x w crop; the affine grid is defined on the whole H x W slice, exactly
+// as aug_resample_kernel<AFFINE> computes it for D = 1 with theta [[a, b, 0, tx], [c, d, 0, ty], [0, 0, 1, 0]]
+template <typename TL>
+__global__ void __launch_bounds__(AUG2D_THREADS) aug2d_gather_kernel(const b200seg_aug2d_row* __restrict__ rows, int max_chunks,
+                                                                    const Aug2dPart* __restrict__ part1, const Aug2dPart* __restrict__ part2,
+                                                                    int h, int w, float* __restrict__ oimg, int64_t* __restrict__ olab) {
+  const int b = blockIdx.y;
+  const b200seg_aug2d_row r = rows[b];
+  const int64_t n = (int64_t)r.H * r.W;
+  const int nch = aug2d_chunks(n);
+  if (nch > max_chunks) {           // statistics were never computed for this slice: make that visible, never guess
+    for (int64_t i = (int64_t)blockIdx.x * AUG2D_THREADS + threadIdx.x; i < (int64_t)h * w; i += (int64_t)gridDim.x * AUG2D_THREADS) {
+      oimg[(int64_t)b * h * w + i] = __int_as_float(0x7fc00000); olab[(int64_t)b * h * w + i] = 0;
+    }
+    return;
+  }
+  Aug2dConsts k;
+  aug2d_consts<true>(part1 + (int64_t)b * max_chunks, part2 + (int64_t)b * max_chunks, nch, (double)n, k);
+  const TL* lab = reinterpret_cast<const TL*>(r.lab);
+  const int64_t HW = (int64_t)h * w;
+  for (int64_t i = (int64_t)blockIdx.x * AUG2D_THREADS + threadIdx.x; i < HW; i += (int64_t)gridDim.x * AUG2D_THREADS) {
+    const int sw = (int)(i % w) + r.crop_x, sh = (int)(i / w) + r.crop_y;
+    const float bx = r.W > 1 ? (2.f * sw) / (float)(r.W - 1) - 1.f : 0.f;
+    const float by = r.H > 1 ? (2.f * sh) / (float)(r.H - 1) - 1.f : 0.f;
+    const float gx = fmaf(bx, r.theta[0], fmaf(by, r.theta[1], fmaf(0.f, 0.f, r.theta[2])));
+    const float gy = fmaf(bx, r.theta[3], fmaf(by, r.theta[4], fmaf(0.f, 0.f, r.theta[5])));
+    const float ix = (gx + 1.f) * 0.5f * (float)(r.W - 1);
+    const float iy = (gy + 1.f) * 0.5f * (float)(r.H - 1);
+    const float fx = floorf(ix), fy = floorf(iy);
+    const int x_0 = (int)fx, y_0 = (int)fy;
+    const float tx = ix - fx, ty = iy - fy;
+    const bool vx0 = (unsigned)x_0 < (unsigned)r.W, vx1 = (unsigned)(x_0 + 1) < (unsigned)r.W;
+    const bool vy0 = (unsigned)y_0 < (unsigned)r.H, vy1 = (unsigned)(y_0 + 1) < (unsigned)r.H;
+    const int64_t base = (int64_t)y_0 * r.W + x_0;
+    const float w00 = (1.f - tx) * (1.f - ty), w01 = tx * (1.f - ty), w10 = (1.f - tx) * ty, w11 = tx * ty;
+    float v = 0.f;
+    if (vy0 && vx0) v += aug2d_y3(r, base, k) * w00;
+    if (vy0 && vx1) v += aug2d_y3(r, base + 1, k) * w01;
+    if (vy1 && vx0) v += aug2d_y3(r, base + r.W, k) * w10;
+    if (vy1 && vx1) v += aug2d_y3(r, base + r.W + 1, k) * w11;
+    oimg[(int64_t)b * HW + i] = v;
+    // mode='nearest': round half to even, zeros outside
+    const int nx = (int)nearbyintf(ix), ny = (int)nearbyintf(iy);
+    int64_t l = 0;
+    if ((unsigned)nx < (unsigned)r.W && (unsigned)ny < (unsigned)r.H) l = (int64_t)lab[(int64_t)ny * r.W + nx];
+    olab[(int64_t)b * HW + i] = l;
   }
 }
 
@@ -372,8 +577,9 @@ extern "C" int b200seg_aug_pointwise(const float* x, float* y, int rows, int64_t
   return B200SEG_OK;
 }
 
-extern "C" int b200seg_aug_gaussian_blur(const float* x, float* y, int C, int D, int H, int W, const float* weights, int ksize,
-                                         void* stats_out, int stats_rows, void* stream) {
+namespace {
+int launch_blur(bool depth, const float* x, float* y, int C, int D, int H, int W, const float* weights, int ksize,
+                void* stats_out, int stats_rows, void* stream) {
   if (!x || !y || !weights || C <= 0 || D <= 0 || H <= 0 || W <= 0 || x == y) return B200SEG_EINVAL;
   if (ksize < 1 || (ksize & 1) == 0) return B200SEG_EINVAL;
   const int R = ksize / 2;
@@ -381,17 +587,59 @@ extern "C" int b200seg_aug_gaussian_blur(const float* x, float* y, int C, int D,
   if (stats_out && stats_rows != 1 && stats_rows != C) return B200SEG_EINVAL;
   BlurW kw;
   for (int i = 0; i < 2 * BR_MAX + 1; ++i) kw.w[i] = i < ksize ? weights[i] : 0.f;
-  const int EZ = BT_Z + 2 * R, EY = BT_Y + 2 * R, EX = BT_X + 2 * R;
+  const int TZ = depth ? BT_Z : 1, RZ = depth ? R : 0;
+  const int EZ = TZ + 2 * RZ, EY = BT_Y + 2 * R, EX = BT_X + 2 * R;
   const size_t smem = sizeof(float) * ((size_t)EZ * EY * EX + (size_t)EZ * EY * BT_X + (size_t)EZ * BT_Y * BT_X);
   static bool attr_set = false;
   if (!attr_set) {
-    B200_CUDA(cudaFuncSetAttribute(aug_blur_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+    B200_CUDA(cudaFuncSetAttribute(aug_blur_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     attr_set = true;
   }
-  const int64_t tiles = (int64_t)C * ((D + BT_Z - 1) / BT_Z) * ((H + BT_Y - 1) / BT_Y) * ((W + BT_X - 1) / BT_X);
+  const int64_t tiles = (int64_t)C * ((D + TZ - 1) / TZ) * ((H + BT_Y - 1) / BT_Y) * ((W + BT_X - 1) / BT_X);
   const int64_t cap = (int64_t)B200SEG_NUM_SMS * 3;
   const int grid = (int)(tiles < cap ? tiles : cap);
-  aug_blur_kernel<<<grid, 256, smem, as_stream(stream)>>>(x, y, C, D, H, W, R, kw, (StatRow*)stats_out, stats_rows);
+  if (depth) aug_blur_kernel<true><<<grid, 256, smem, as_stream(stream)>>>(x, y, C, D, H, W, R, kw, (StatRow*)stats_out, stats_rows);
+  else aug_blur_kernel<false><<<grid, 256, smem, as_stream(stream)>>>(x, y, C, D, H, W, R, kw, (StatRow*)stats_out, stats_rows);
   B200_CHECK_LAUNCH("aug_blur_kernel");
+  return B200SEG_OK;
+}
+}  // namespace
+
+extern "C" int b200seg_aug_gaussian_blur(const float* x, float* y, int C, int D, int H, int W, const float* weights, int ksize,
+                                         void* stats_out, int stats_rows, void* stream) {
+  return launch_blur(true, x, y, C, D, H, W, weights, ksize, stats_out, stats_rows, stream);
+}
+
+extern "C" int b200seg_aug_gaussian_blur2d(const float* x, float* y, int C, int H, int W, const float* weights, int ksize,
+                                           void* stats_out, int stats_rows, void* stream) {
+  return launch_blur(false, x, y, C, 1, H, W, weights, ksize, stats_out, stats_rows, stream);
+}
+
+extern "C" size_t b200seg_aug2d_workspace(int B, int64_t max_elems) {
+  if (B <= 0 || max_elems <= 0) return 0;
+  return (size_t)2 * B * (size_t)((max_elems + AUG2D_CHUNK - 1) / AUG2D_CHUNK) * sizeof(Aug2dPart);
+}
+
+extern "C" int b200seg_aug2d_train(const void* rows, int B, int64_t max_elems, int lab_bytes, int h, int w, float* out_img,
+                                   int64_t* out_lab, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!rows || !out_img || !out_lab || !workspace || B <= 0 || max_elems <= 0 || h <= 0 || w <= 0) return B200SEG_EINVAL;
+  if (B > 65535) return B200SEG_EUNSUPPORTED;
+  if (lab_bytes != 1 && lab_bytes != 8) return B200SEG_EINVAL;
+  if (workspace_bytes < b200seg_aug2d_workspace(B, max_elems)) return B200SEG_EINVAL;
+  const int max_chunks = (int)((max_elems + AUG2D_CHUNK - 1) / AUG2D_CHUNK);
+  const b200seg_aug2d_row* r = (const b200seg_aug2d_row*)rows;
+  Aug2dPart* p1 = (Aug2dPart*)workspace;
+  Aug2dPart* p2 = p1 + (size_t)B * max_chunks;
+  cudaStream_t st = as_stream(stream);
+  const dim3 gs(max_chunks, B);
+  aug2d_stats_kernel<1><<<gs, AUG2D_THREADS, 0, st>>>(r, max_chunks, p1, p2);
+  B200_CHECK_LAUNCH("aug2d_stats_kernel<1>");
+  aug2d_stats_kernel<2><<<gs, AUG2D_THREADS, 0, st>>>(r, max_chunks, p1, p2);
+  B200_CHECK_LAUNCH("aug2d_stats_kernel<2>");
+  const int64_t per = ((int64_t)h * w + AUG2D_THREADS - 1) / AUG2D_THREADS;
+  const dim3 gg((unsigned)(per < 65535 ? per : 65535), B);
+  if (lab_bytes == 1) aug2d_gather_kernel<uint8_t><<<gg, AUG2D_THREADS, 0, st>>>(r, max_chunks, p1, p2, h, w, out_img, out_lab);
+  else aug2d_gather_kernel<int64_t><<<gg, AUG2D_THREADS, 0, st>>>(r, max_chunks, p1, p2, h, w, out_img, out_lab);
+  B200_CHECK_LAUNCH("aug2d_gather_kernel");
   return B200SEG_OK;
 }

@@ -558,6 +558,40 @@ int b200seg_aug_pointwise(const float* x, float* y, int rows, int64_t n, int op,
                           uint64_t seed, void* stream);
 int b200seg_aug_gaussian_blur(const float* x, float* y, int C, int D, int H, int W, const float* weights,
                               int ksize, void* stats_out, int stats_rows, void* stream);
+/* aug_gaussian_blur2d: gaussian_blur on a [1,C,H,W] image (F.conv2d with the normalised k x k kernel, which is
+ *   the outer product of the normalised 1-D weights), zero padding k//2; otherwise as aug_gaussian_blur. */
+int b200seg_aug_gaussian_blur2d(const float* x, float* y, int C, int H, int W, const float* weights, int ksize,
+                                void* stats_out, int stats_rows, void* stream);
+
+/* ---------------------------------------------------------------------------
+ * Batched 2-D training branch (training/dataset/dim2/dataset_acdc.py:128-142) for B ragged slices:
+ *   y1 = x + noise_std*N(0,1) + beta        gaussian_noise (Philox keyed by noise_key, counter = element / 4,
+ *                                           the stream aug_pointwise op 5 draws) and brightness_additive
+ *   y2 = ((y1 - min1)/rng1)^gamma*rng1 + min1,  y3 = (y2 - mean2)/std2*std1 + mean1
+ *                                           gamma(retain_stats=True); statistics of the whole slice, std unbiased
+ *   random_scale_rotate_translate_2d with the 2x3 theta (F.affine_grid / F.grid_sample over the whole H x W slice,
+ *   align_corners=True, bilinear image / nearest label, zeros padding), of which only the h x w crop at
+ *   (crop_y, crop_x) is produced (crop_2d).
+ * rows: DEVICE array of B b200seg_aug2d_row (88 bytes each).  img fp32 [H][W]; lab uint8 (lab_bytes = 1) or
+ * int64 (8) [H][W]; y1 (nullable) receives y1, [H][W] fp32.  max_elems >= every H*W.  out_img fp32 [B][h][w],
+ * out_lab int64 [B][h][w].  Three launches whatever B; statistics stay on the device, reduced in a fixed order
+ * without atomics, so a given table always gives the same bits.
+ * workspace: b200seg_aug2d_workspace(B, max_elems) bytes of device memory.
+ * ------------------------------------------------------------------------- */
+typedef struct {
+  const float* img;
+  const void* lab;
+  float* y1;
+  int H, W;
+  uint64_t noise_key;
+  float noise_std, beta, gamma;
+  float theta[6];          /* row-major 2x3, as handed to F.affine_grid */
+  int crop_y, crop_x;
+  int reserved;
+} b200seg_aug2d_row;
+size_t b200seg_aug2d_workspace(int B, int64_t max_elems);
+int b200seg_aug2d_train(const void* rows, int B, int64_t max_elems, int lab_bytes, int h, int w, float* out_img,
+                        int64_t* out_lab, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------
  * Attention-UNet gate (SURVEY.md 8f.4), model/dim3/attention_unet_utils.py:7-37.  With
