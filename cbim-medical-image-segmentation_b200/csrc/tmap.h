@@ -2,11 +2,15 @@
 // libcuda: cuTensorMapEncodeTiled is fetched through the runtime's driver-entry-point query.
 //
 // An activation slice x[b][d][h][w][coff : coff + C] (fp16, row pitch ld) is described as the 5-D tensor
-//   dim0 = 8 channels (16 B, contiguous)      dim1 = w (stride ld*2 B)      dim2 = h (stride W*ld*2)
-//   dim3 = channel plane c/8 (stride 16 B)    dim4 = b*D + d (stride H*W*ld*2)
-// so that ONE cp.async.bulk.tensor box {8, bw, bh, planes, 1} lands in shared memory as [plane][bh x bw voxels][8 ch] —
-// exactly the no-swizzle wgmma operand image conv_tc.cu / wgrad_tc.cu consume (K-major for the forward GEMM, MN-major
-// for the weight gradient) — with out-of-volume voxels (conv padding, ragged tiles) zero-filled by the TMA unit.
+//   dim0 = g channels (2g B, contiguous)      dim1 = w (stride ld*2 B)      dim2 = h (stride W*ld*2)
+//   dim3 = channel group c/g (stride 2g B)    dim4 = b*D + d (stride H*W*ld*2)
+// so that ONE cp.async.bulk.tensor box {g, bw, bh, groups, 1} lands in shared memory as [group][bh x bw voxels][g ch],
+// with out-of-volume voxels (conv padding, ragged tiles) zero-filled by the TMA unit.  The group width g picks the image:
+//   g = 8:  16-byte channel planes, no swizzle — the wgmma operand image of conv_tc.cu (K-major) and of wgrad_tc.cu's
+//           plane path (MN-major);
+//   g = 32 / 64: one 64- / 128-byte row of channels per voxel, stored SWIZZLE_64B / SWIZZLE_128B (the 16-byte chunk j of
+//           the row at shared address A lands at chunk j ^ ((A >> 7) & 3 / 7)) — the MN-major swizzled wgmma image of
+//           wgrad_tc.cu's row path.  The destination must be 512- / 1024-byte aligned.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -31,18 +35,21 @@ static inline b200seg_encode_tiled_fn b200seg_encode_tiled() {
 }
 
 // returns false when the map cannot be built (driver entry point missing / shape rejected): callers use their
-// cp.async staging path then
+// cp.async staging path then.  box_groups counts groups of ch_box channels (8, 32 or 64; C must be a multiple of it).
 static inline bool b200seg_make_act_tmap(CUtensorMap* m, const void* base_fp16, int ld, int coff, int C, int BD, int H, int W,
-                                         int box_w, int box_h, int box_planes) {
+                                         int box_w, int box_h, int box_groups, int ch_box = 8) {
   b200seg_encode_tiled_fn enc = b200seg_encode_tiled();
-  if (!enc || (C % 8) || (ld % 8) || (coff % 8)) return false;
+  if (!enc || (C % ch_box) || (ld % 8) || (coff % 8)) return false;
+  if (ch_box != 8 && ch_box != 32 && ch_box != 64) return false;
   const char* base = reinterpret_cast<const char*>(base_fp16) + (size_t)coff * 2;
   if (reinterpret_cast<uintptr_t>(base) & 15) return false;
-  if (box_w > 256 || box_h > 256 || box_planes > 256) return false;
-  cuuint64_t dims[5] = {8, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)(C / 8), (cuuint64_t)BD};
-  cuuint64_t strides[4] = {(cuuint64_t)ld * 2, (cuuint64_t)W * ld * 2, 16, (cuuint64_t)H * W * ld * 2};
-  cuuint32_t box[5] = {8, (cuuint32_t)box_w, (cuuint32_t)box_h, (cuuint32_t)box_planes, 1};
+  if (box_w > 256 || box_h > 256 || box_groups > 256) return false;
+  const CUtensorMapSwizzle swz = ch_box == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : ch_box == 32 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                                                          : CU_TENSOR_MAP_SWIZZLE_NONE;
+  cuuint64_t dims[5] = {(cuuint64_t)ch_box, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)(C / ch_box), (cuuint64_t)BD};
+  cuuint64_t strides[4] = {(cuuint64_t)ld * 2, (cuuint64_t)W * ld * 2, (cuuint64_t)ch_box * 2, (cuuint64_t)H * W * ld * 2};
+  cuuint32_t box[5] = {(cuuint32_t)ch_box, (cuuint32_t)box_w, (cuuint32_t)box_h, (cuuint32_t)box_groups, 1};
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<char*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+             swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }

@@ -7,13 +7,19 @@
 // GEMM view per CTA: D_tap[128 co][N ci] += dy^T[128 co x 128 voxels] * a_tap[128 voxels x N ci] for a GROUP of
 // in-plane taps of one depth offset zd; K = voxels, accumulated over every voxel tile the CTA owns, so the
 // accumulators stay in registers for the CTA's whole life (G*N <= 192 columns) and there is ONE epilogue.
-//   * both operands are staged as [channel/8][voxel][8 ch] — the same image conv_tc.cu uses — and read by
-//     wgmma as MN-major no-swizzle matrices (core matrix = 8 voxels x 8 channels, 128 B):
-//     A = dy tile (16x8 voxels), B = halo tile of `a` ((16+kh-1)x(8+kw-1) voxels); a tap is a shifted
-//     B descriptor, exactly like the forward kernel.
+//   * A = dy tile (16x8 voxels), B = halo tile of `a` ((16+kh-1)x(8+kw-1) voxels), both read by wgmma as MN-major
+//     matrices; a tap is a B descriptor shifted by whole voxels.  Each operand is staged in one of two images:
+//       rows   — one 64- or 128-byte row of 32 / 64 channels per voxel, [group][voxel][32 or 64 ch], stored
+//                SWIZZLE_64B / SWIZZLE_128B (tmap.h) and read through swizzled descriptors (SBO = 8 voxel rows).
+//                Used for dy when min(Cout, 128) is 32, 64 or 128 (Cout a multiple of 64 above 64) and for x when the
+//                Cin tile is 32, 64 or 96 (three 32-channel groups);
+//       planes — [channel/8][voxel][8 ch], the image conv_tc.cu uses, read through no-swizzle descriptors (core matrix
+//                = 8 voxels x 8 channels, 128 B), for every other width.
+//     A row image moves a voxel's channels as one 64- or 128-byte TMA line instead of 4 or 8 16-byte ones.  Either way
+//     the MMAs, their operands and their K order are the same, so dW does not depend on the image.
 //   * both operands arrive by tensor TMA: per stage one elected thread issues one box for the dy tile and one for the
-//     x halo tile (tmap.h; out-of-volume voxels are zero-filled by the TMA unit) onto the stage's LAND barrier, as soon
-//     as the consumers hand the slot back, so every free slot of the ring is in flight.
+//     x halo tile (three at a Cin tile of 96; tmap.h; out-of-volume voxels are zero-filled by the TMA unit) onto the
+//     stage's LAND barrier, as soon as the consumers hand the slot back, so every free slot of the ring is in flight.
 //   * `a` is never materialised by a separate pass: when x needs InstanceNorm-normalise + activation, the other loader
 //     warps apply it in place in shared memory once a stage has landed (zero-filled padding voxels stay zero, as in
 //     conv_tc.cu's forward loader) and publish FULL; raw x is consumed straight off LAND.
@@ -52,8 +58,9 @@ constexpr int kRegsLaunch = 128, kRegsConsumer = 152, kRegsLoad = 104;
 static_assert(2 * 128 * kRegsConsumer + 2 * 128 * kRegsLoad <= kThreads * kRegsLaunch, "register split exceeds the CTA pool");
 
 struct WgParams {
-  alignas(64) CUtensorMap tm_dy;           // dy as {8 ch, w, h, plane, b*D+d}, box {8, TW, TS, min(Cout, MT)/8}
-  alignas(64) CUtensorMap tm_x;            // x likewise, box {8, HALO_W, HALO_H, NTC/8}
+  alignas(64) CUtensorMap tm_dy;           // dy as {g ch, w, h, group, b*D+d}, box {dy_ch, TW, TS, min(Cout, MT)/dy_ch}
+  alignas(64) CUtensorMap tm_x;            // x likewise: planes {8, HALO_W, HALO_H, NTC/8}, rows x_boxes x {x_ch, .., 1}
+  uint64_t dy_desc, x_desc;                // wgmma descriptor templates (layout, LBO, SBO) of the two staged images
   const double* x_stats; float eps; int act;   // x is normalised + activated in shared memory when x_stats / act
   const float* x_affine; int per_channel;      // or transformed per channel (conv_args.h); the table is then [NTC]
   float* dw;
@@ -61,7 +68,8 @@ struct WgParams {
   int B, D, H, W, Cin, Cout, kd, kh, kw;
   int NTC, ci_tiles, co_tiles, ngroups, gbase, grem, S;
   int TS, halves;                          // voxel rows per stage: TH (whole tiles) or TH/2 (two stages per tile)
-  int HALO_H, HALO_W, nvox_h, a_plane, dy_plane, a_bytes, dy_bytes, stage_bytes, NS;
+  int dy_ch, x_ch, x_boxes;                // channels per staged group (8 = planes, 32 / 64 = rows); x boxes per stage
+  int HALO_H, HALO_W, nvox_h, a_plane, dy_plane, a_bytes, dy_bytes, stage_bytes, NS;   // *_plane: group stride
   int tiles_h, tiles_w, nvt;
   int smem_bar_off, smem_norm_off;
 };
@@ -138,13 +146,14 @@ struct VtCursor {
 };
 
 // ---- TMA producer (one thread): per stage, once both consumers have handed the slot back, one box of dy
-// {8 ch, TW, TS, Cout planes} and one box of the x halo {8 ch, HALO_W, HALO_H, NTC/8 planes}, both completing on LAND.
-// Each box lands as [plane][voxel][8 ch] with dense planes; out-of-volume voxels and output channels past Cout are
-// zero-filled and counted in the transaction bytes like any other.
+// {dy_ch, TW, TS, co_max/dy_ch groups} and the x halo as one box {8 ch, HALO_W, HALO_H, NTC/8 planes} (planes) or
+// x_boxes boxes {x_ch, HALO_W, HALO_H, 1} a_plane apart (rows), all completing on LAND.  Out-of-volume voxels and output
+// channels past Cout are zero-filled and counted in the transaction bytes like any other.
 __device__ __forceinline__ void tma_producer(const WgParams& p, const Job& job, uint8_t* smem, const Bars& bars) {
   const int ph = p.kh / 2, pw = p.kw / 2, zoff = job.zd - p.kd / 2;
-  const int co_p0 = job.co_tile * (MT / 8), ci_p0 = job.ci_tile * (p.NTC / 8);
-  const uint32_t stage_tx = (uint32_t)(p.dy_bytes + (p.NTC / 8) * p.a_plane);
+  const int co_g0 = job.co_tile * (MT / p.dy_ch), ci_g0 = job.ci_tile * (p.NTC / p.x_ch);
+  const int x_box_groups = p.NTC / p.x_ch / p.x_boxes;
+  const uint32_t stage_tx = (uint32_t)(p.dy_bytes + p.NTC * p.nvox_h * 2);
   VtWalk vw; vw.init(p);
   VtCursor c; c.init(vw, p, job.s, zoff);
   Ring r; r.init(p.NS);
@@ -152,14 +161,19 @@ __device__ __forceinline__ void tma_producer(const WgParams& p, const Job& job, 
     mbar_wait(bars.empty(r.idx), r.phase ^ 1);
     const uint32_t sdy = smem_u32(smem + r.idx * p.stage_bytes);
     mbar_arrive_expect_tx(bars.land(r.idx), stage_tx);
-    tma_load_5d(sdy, &p.tm_dy, bars.land(r.idx), 0, c.w0(), c.h0(p), co_p0, c.b * p.D + c.d);
-    tma_load_5d(sdy + (uint32_t)p.dy_bytes, &p.tm_x, bars.land(r.idx), 0, c.w0() - pw, c.h0(p) - ph, ci_p0, c.b * p.D + c.din);
+    tma_load_5d(sdy, &p.tm_dy, bars.land(r.idx), 0, c.w0(), c.h0(p), co_g0, c.b * p.D + c.d);
+    for (int i = 0; i < p.x_boxes; ++i)
+      tma_load_5d(sdy + (uint32_t)(p.dy_bytes + i * p.a_plane), &p.tm_x, bars.land(r.idx), 0, c.w0() - pw, c.h0(p) - ph,
+                  ci_g0 + i * x_box_groups, c.b * p.D + c.din);
     r.advance();
   }
 }
 
 // ---- in-place InstanceNorm-normalise + activation of each landed x halo tile (only when x needs it).  Thread owns
-// plane (xt % cpv) and the halo voxels v0, v0 + vstep, ... of it; zero-filled padding voxels stay zero.
+// the 8-channel chunk c8 = xt % cpv of the halo voxels v0, v0 + vstep, ...; zero-filled padding voxels stay zero.  In a
+// row image the chunk sits in group c8 / (x_ch/8) at position j ^ phase(row), j = c8 % (x_ch/8), where the phase is
+// the row's shared-address bits 7.. (the TMA swizzle; the stage and every group start are aligned to its repeat); in
+// the plane image it is plane c8 and the phase mask is 0.
 __device__ __forceinline__ void transform_role(const WgParams& p, const Job& job, uint8_t* smem, const float2* s_norm, const Bars& bars) {
   const int xt = threadIdx.x - (kLoadWarp0 + 1) * 32;
   const int ph = p.kh / 2, pw = p.kw / 2, zoff = job.zd - p.kd / 2;
@@ -167,6 +181,9 @@ __device__ __forceinline__ void transform_role(const WgParams& p, const Job& job
   const int vstep = kXformThreads / cpv;
   const bool active = xt < vstep * cpv;
   const int c8 = xt % cpv, v0 = xt / cpv;
+  const int gch = p.x_ch / 8, row_bytes = p.x_ch * 2;
+  const uint32_t chunk = (uint32_t)(c8 % gch), phase_mask = p.x_ch == 64 ? 7u : p.x_ch == 32 ? 3u : 0u;
+  const uint32_t group_off = (uint32_t)(p.dy_bytes + (c8 / gch) * p.a_plane);
   const int sh = vstep / p.HALO_W, sw = vstep % p.HALO_W;
   const int hh0 = v0 / p.HALO_W, ww0 = v0 % p.HALO_W;
   const bool relu = p.act == B200SEG_ACT_RELU;
@@ -177,7 +194,7 @@ __device__ __forceinline__ void transform_role(const WgParams& p, const Job& job
   for (; c.valid(p); c.next(vw, p, zoff)) {
     mbar_wait(bars.land(r.idx), r.phase);
     if (active) {
-      uint8_t* sp = smem + r.idx * p.stage_bytes + p.dy_bytes + c8 * p.a_plane;
+      uint32_t off = (uint32_t)(r.idx * p.stage_bytes) + group_off + (uint32_t)(v0 * row_bytes);
       float sc[8], sf[8];                          // x*sc + sf: (x - mean) * rstd, or the per-channel transform
       const float2* tb = s_norm + (p.per_channel ? 0 : c.b * p.NTC) + c8 * 8;
 #pragma unroll
@@ -191,9 +208,10 @@ __device__ __forceinline__ void transform_role(const WgParams& p, const Job& job
       for (int v = v0; v < p.nvox_h; v += vstep) {
         const int h = hb + hh, w = wb + ww;
         if ((unsigned)h < (unsigned)p.H && (unsigned)w < (unsigned)p.W) {      // padding voxels stay zero
-          uint4* chunk = reinterpret_cast<uint4*>(sp + v * 16);
-          *chunk = relu ? norm_act8<true>(*chunk, sc, sf, slope) : norm_act8<false>(*chunk, sc, sf, slope);
+          uint4* q = reinterpret_cast<uint4*>(smem + off + ((chunk ^ ((off >> 7) & phase_mask)) << 4));
+          *q = relu ? norm_act8<true>(*q, sc, sf, slope) : norm_act8<false>(*q, sc, sf, slope);
         }
+        off += (uint32_t)(vstep * row_bytes);
         hh += sh; ww += sw;
         if (ww >= p.HALO_W) { ww -= p.HALO_W; ++hh; }
       }
@@ -240,22 +258,20 @@ __device__ __forceinline__ void idle_consumer_role(const WgParams& p, const Job&
 template <int NTC, int NTAPS, int KS>
 __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job, int wg, int tid, uint8_t* smem, const Bars& bars) {
   const int zoff = job.zd - p.kd / 2;
-  // dy^T as the A operand: MN-major (lbo = next 8 voxels, sbo = next channel plane); x halo tile as the B operand:
-  // MN-major (lbo = next halo row of voxels, sbo = next channel plane), a tap = start shifted by whole voxel slots
-  const uint64_t dy_tmpl = make_desc(0, 128u, (uint32_t)p.dy_plane);
-  const uint64_t a_tmpl = make_desc(0, (uint32_t)p.HALO_W * 16u, (uint32_t)p.a_plane);
-  const uint32_t dy_kstep = 16u;                                       // 16 voxels = 256 B
-  const uint32_t a_kstep = 2u * (uint32_t)p.HALO_W;                    // two halo rows of voxels per K=16 step
+  // dy^T as the A operand, the x halo tile as the B operand, both MN-major (fill_params builds the descriptor
+  // templates); every shift below is a whole number of voxels, one voxel = x_ch / 8 (or dy_ch / 8) 16-byte units
+  const uint32_t dy_vox16 = (uint32_t)p.dy_ch >> 3, x_vox16 = (uint32_t)p.x_ch >> 3;
+  const uint32_t dy_kstep = 16u * dy_vox16;                            // 16 voxels per K=16 step
+  const uint32_t a_kstep = 2u * (uint32_t)p.HALO_W * x_vox16;          // two halo rows of voxels per K=16 step
   const uint32_t stage16 = (uint32_t)p.stage_bytes >> 4, dy16 = (uint32_t)p.dy_bytes >> 4;
   const uint32_t smem16 = smem_u32(smem) >> 4;
-  const uint32_t dy_wg16 = (uint32_t)(wg * 8 * p.dy_plane) >> 4;
-  // start of each tap's B operand in the staged halo tile, in 16-byte voxel slots: taps run along w, then wrap to the
-  // next halo row
+  const uint32_t dy_wg16 = (uint32_t)(wg * (64 / p.dy_ch) * p.dy_plane) >> 4;     // the warpgroup's 64 output channels
+  // start of each tap's B operand in the staged halo tile: taps run along w, then wrap to the next halo row
   uint32_t tap_off[NTAPS];
 #pragma unroll
   for (int g = 0; g < NTAPS; ++g) {
     const int t = job.tap0 + g;
-    tap_off[g] = (uint32_t)((t / p.kw) * p.HALO_W + t % p.kw);
+    tap_off[g] = (uint32_t)((t / p.kw) * p.HALO_W + t % p.kw) * x_vox16;
   }
   float acc[NTAPS][NTC / 2];
   VtWalk vw; vw.init(p);
@@ -266,20 +282,21 @@ __device__ __forceinline__ void consumer_role(const WgParams& p, const Job& job,
   uint32_t accumulate = 0;
   for (; c.valid(p); c.next(vw, p, zoff)) {
     mbar_wait(bars.ready(r.idx), r.phase);
-    const uint64_t da0 = dy_tmpl + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy_wg16);
-    const uint64_t db0 = a_tmpl + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy16);
+    const uint64_t da0 = p.dy_desc + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy_wg16);
+    const uint64_t db0 = p.x_desc + (uint64_t)(smem16 + (uint32_t)r.idx * stage16 + dy16);
 #pragma unroll
     for (int g = 0; g < NTAPS; ++g) wgmma_fence_operands(acc[g]);
     wgmma_fence();
 #pragma unroll
     for (int g = 0; g < NTAPS; ++g) {
-      uint64_t db = db0 + (uint64_t)tap_off[g];
-      // opaque per stage: otherwise ptxas hoists all NTAPS x 8 loop-invariant B offsets into registers and spills
-      asm volatile("" : "+l"(db));
+      uint64_t db = db0 + (uint64_t)tap_off[g], da = da0;
 #pragma unroll
-      for (int j = 0; j < KS; ++j)
-        Wgmma<NTC, 1, 1>::mma(acc[g], da0 + (uint64_t)((uint32_t)j * dy_kstep), db + (uint64_t)((uint32_t)j * a_kstep),
-                              accumulate | (uint32_t)(j > 0));
+      for (int j = 0; j < KS; ++j) {
+        // opaque per step: otherwise ptxas hoists all NTAPS x KS loop-invariant offsets into registers and spills
+        asm volatile("" : "+l"(da), "+l"(db));
+        Wgmma<NTC, 1, 1>::mma(acc[g], da, db, accumulate | (uint32_t)(j > 0));
+        da += dy_kstep; db += a_kstep;
+      }
     }
     wgmma_commit();
     wgmma_wait<1>();                               // the group before this one has retired: its stage is free
@@ -417,19 +434,39 @@ bool fill_params(const WgradArgs& a, WgParams& p) {
   auto size_ring = [&](int ts) {
     p.TS = ts; p.halves = TH / ts;
     p.HALO_H = ts + a.kh - 1; p.nvox_h = p.HALO_H * p.HALO_W;
-    p.a_plane = p.nvox_h * 16;                 // TMA boxes land with dense planes
-    p.dy_plane = ts * TW * 16;
-    p.a_bytes = (p.NTC / 8) * p.a_plane; p.a_bytes = (p.a_bytes + 127) / 128 * 128;
-    p.dy_bytes = (co_max / 8) * p.dy_plane;    // a multiple of 1024: the `a` box starts 128-byte aligned
+    // TMA boxes land with dense groups; a 32-channel row group starts on the 512-byte SWIZZLE_64B repeat
+    p.a_plane = p.nvox_h * p.x_ch * 2;
+    if (p.x_ch == 32) p.a_plane = (p.a_plane + 511) / 512 * 512;
+    p.dy_plane = ts * TW * p.dy_ch * 2;
+    // a multiple of 1024 (co_max >= 8, ts >= 8): the `a` box starts 1024-byte aligned.  With a row image in the stage
+    // every stage starts on the 1024-byte SWIZZLE_128B repeat as well.
+    p.dy_bytes = (co_max / p.dy_ch) * p.dy_plane;
+    const int align = p.dy_ch != 8 || p.x_ch != 8 ? 1024 : 128;
+    p.a_bytes = (p.NTC / p.x_ch) * p.a_plane; p.a_bytes = (p.a_bytes + align - 1) / align * align;
     p.stage_bytes = p.a_bytes + p.dy_bytes;
-    const int span = (co_max + 63) / 64 * 8 * p.dy_plane;
+    // a plane-image A descriptor spans 8 whole planes per warpgroup and may read past the staged ones; a row image's
+    // descriptor stays inside them (Cout 32: its second 32-channel atom is the first one again, LBO = 0)
+    const int span = p.dy_ch == 8 ? (co_max + 63) / 64 * 8 * p.dy_plane : 0;
     tail = span > p.stage_bytes ? span - p.stage_bytes : 0;
     p.NS = (227 * 1024 - 2048 - tail - norm_bytes) / p.stage_bytes;
     if (p.NS > kMaxStages) p.NS = kMaxStages;
   };
   // whole 16x8 tiles, or two 8-row halves per tile where fewer than 4 whole tiles fit
-  size_ring(TH);
-  if (p.NS < 4) size_ring(TH / 2);
+  auto size = [&](int dy_ch, int x_ch) {
+    p.dy_ch = dy_ch; p.x_ch = x_ch; p.x_boxes = x_ch == 8 ? 1 : p.NTC / x_ch;
+    size_ring(TH);
+    if (p.NS < 4) size_ring(TH / 2);
+  };
+  // row images: dy where the M tile is whole 32- or 64-channel groups of real channels, x at Cin tiles of 32, 64, 96 —
+  // unless aligning the stages to the swizzle repeat would cost the ring a stage (a row image next to a plane image)
+  size(8, 8);
+  const int ns_planes = p.NS, ts_planes = p.TS;
+  const int dy_ch = co_max == 32 ? 32 : (co_max == 64 || (co_max == MT && a.Cout % 64 == 0)) ? 64 : 8;
+  const int x_ch = p.NTC == 64 ? 64 : (p.NTC == 32 || p.NTC == 96) ? 32 : 8;
+  if (dy_ch != 8 || x_ch != 8) {
+    size(dy_ch, x_ch);
+    if (p.NS != ns_planes || p.TS != ts_planes) size(8, 8);
+  }
   if (p.NS < 2) return false;
   p.tiles_h = (a.H + TH - 1) / TH; p.tiles_w = (a.W + TW - 1) / TW;
   const int64_t nvt = (int64_t)a.B * a.D * p.tiles_h * p.tiles_w;
@@ -439,6 +476,20 @@ bool fill_params(const WgradArgs& a, WgParams& p) {
   int S = (int)(B200SEG_NUM_SMS / jobs); if (S < 1) S = 1;
   if (S > p.nvt) S = p.nvt;
   p.S = S;
+  // wgmma descriptor templates: the layout type in bits 62-63 (0 none, 1 SWIZZLE_128B, 2 SWIZZLE_64B), LBO and SBO.
+  // MN-major no swizzle: LBO = next 8 voxels (K), SBO = next 8-channel plane (M / N).  MN-major swizzled: LBO = next
+  // channel group (M / N), SBO = next 8 voxel rows (K).  The base-offset field stays 0 although a tap or K step starts
+  // an operand mid-way through the 8-row swizzle atom: the tensor core XORs each row's chunks with bits 7.. of the row's
+  // own shared address, as the TMA unit does when it stores them, so the start address alone places every row (checked
+  // bit for bit against the plane image on H100; setting the field to the start's phase corrupts dW).
+  auto layout = [](int ch) { return (uint64_t)(ch == 64 ? 1 : ch == 32 ? 2 : 0) << 62; };
+  auto desc = [](uint32_t lbo, uint32_t sbo) {
+    return (uint64_t)((lbo >> 4) & 0x3FFF) << 16 | (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
+  };
+  p.dy_desc = layout(p.dy_ch) | (p.dy_ch == 8 ? desc(128u, (uint32_t)p.dy_plane) : desc(0u, 8u * 2u * p.dy_ch));
+  // B: the next 8 voxels of a K step lie one halo row on
+  p.x_desc = layout(p.x_ch) | (p.x_ch == 8 ? desc((uint32_t)p.HALO_W * 16u, (uint32_t)p.a_plane)
+                                            : desc((uint32_t)p.a_plane, (uint32_t)p.HALO_W * 2u * p.x_ch));
   int off = p.NS * p.stage_bytes + tail;
   off = (off + 15) / 16 * 16;
   p.smem_bar_off = off; off += 3 * p.NS * 8;
@@ -475,8 +526,10 @@ int conv3d_wgrad_tc(const WgradArgs& a, int dtype, void* workspace, size_t ws_by
   fill_params(a, p);
   // the alignment conditions of conv3d_wgrad_tc_supported are the ones TMA needs; only a missing driver entry point
   // can make this fail
-  if (!b200seg_make_act_tmap(&p.tm_dy, a.dy, a.dy_ld, a.dy_coff, a.Cout, a.B * a.D, a.H, a.W, TW, p.TS, (a.Cout < MT ? a.Cout : MT) / 8) ||
-      !b200seg_make_act_tmap(&p.tm_x, a.x, a.x_ld, a.x_coff, a.Cin, a.B * a.D, a.H, a.W, p.HALO_W, p.HALO_H, p.NTC / 8))
+  if (!b200seg_make_act_tmap(&p.tm_dy, a.dy, a.dy_ld, a.dy_coff, a.Cout, a.B * a.D, a.H, a.W, TW, p.TS,
+                             (a.Cout < MT ? a.Cout : MT) / p.dy_ch, p.dy_ch) ||
+      !b200seg_make_act_tmap(&p.tm_x, a.x, a.x_ld, a.x_coff, a.Cin, a.B * a.D, a.H, a.W, p.HALO_W, p.HALO_H,
+                             p.NTC / p.x_ch / p.x_boxes, p.x_ch))
     return B200SEG_ECUDA;
   p.x_stats = a.x_stats; p.eps = a.eps; p.act = a.act;
   p.x_affine = a.x_affine; p.per_channel = a.per_channel;

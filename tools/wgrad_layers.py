@@ -6,9 +6,10 @@ one bench.py training step, fused conv1|shortcut shapes included.
 Runs one training step of the workload with ops.conv3d_wgrad wrapped to record each call's shape, operand layout
 (ld / channel offset) and input transform, then times each distinct call with CUDA events: the C entry point back to
 back into preallocated dW / workspace, the split-K slice sum included.  Per shape it prints the calls per step, the
-kernel's job split (jobs, split-K factor S, CTAs), its ring (stages NS; whole 16x8 tiles or 8-row halves), the bytes
-the kernel stages into shared memory per call (computed from the shape), the time, TFLOP/s, and the FLOP-weighted sum
-per step.  The launch configuration is the host-side choice of csrc/wgrad_tc.cu (pick_ntc / fill_params), mirrored
+kernel's job split (jobs, split-K factor S, CTAs), its ring (stages NS; whole 16x8 tiles or 8-row halves), the staged
+image of x and dy (r32 / r64: swizzled rows of 32 / 64 channels per voxel, p8: 16-byte channel planes), the bytes and
+TMA lines (one innermost box row each) the kernel stages into shared memory per call (computed from the shape), the
+time, TFLOP/s, the staged rate per CTA, and the FLOP-weighted sum per step.  The launch configuration is the host-side choice of csrc/wgrad_tc.cu (pick_ntc / fill_params), mirrored
 here.  The card name and power limit are printed with the numbers."""
 import argparse
 import json
@@ -46,19 +47,36 @@ def plan(cin, cout, k, B, D, H, W):
     ngroups = -(-taps_hw // g)
     co_max = min(cout, MT)
 
-    def ring(ts):
+    def ring(ts, dy_ch, x_ch):
+        rows = dy_ch != 8 or x_ch != 8
         halo_w, halo_h = 8 + kw - 1, ts + kh - 1
-        a_box = ntc // 8 * halo_h * halo_w * 16
-        dy_box = co_max // 8 * ts * 8 * 16
-        stage = -(-a_box // 128) * 128 + dy_box
-        tail = max(0, -(-co_max // 64) * 8 * ts * 8 * 16 - stage)
-        return min((SMEM - tail - B * ntc * 8) // stage, MAX_STAGES), a_box + dy_box
+        a_group = halo_h * halo_w * x_ch * 2
+        if x_ch == 32:
+            a_group = -(-a_group // 512) * 512
+        align = 1024 if rows else 128
+        a_box = ntc * halo_h * halo_w * 2
+        dy_box = co_max * ts * 8 * 2
+        stage = -(-(ntc // x_ch * a_group) // align) * align + dy_box
+        tail = max(0, -(-co_max // 64) * 8 * ts * 8 * 16 - stage) if dy_ch == 8 else 0
+        lines = halo_h * halo_w * (ntc // x_ch) + ts * 8 * (co_max // dy_ch)
+        return min((SMEM - tail - B * ntc * 8) // stage, MAX_STAGES), a_box + dy_box, lines
 
-    ts = 16
-    ns, stage_tx = ring(ts)
-    if ns < 4:
-        ts = 8
-        ns, stage_tx = ring(ts)
+    def size(dy_ch, x_ch):
+        ts = 16
+        r = ring(ts, dy_ch, x_ch)
+        if r[0] < 4:
+            ts = 8
+            r = ring(ts, dy_ch, x_ch)
+        return (ts, dy_ch, x_ch) + r
+
+    # row images unless they cost the ring a stage (a row image next to a plane image)
+    planes = size(8, 8)
+    dy_ch = 32 if co_max == 32 else 64 if (co_max == 64 or (co_max == MT and cout % 64 == 0)) else 8
+    x_ch = 64 if ntc == 64 else 32 if ntc in (32, 96) else 8
+    pick = size(dy_ch, x_ch)
+    if pick[:4:3] != planes[:4:3]:
+        pick = planes
+    ts, dy_ch, x_ch, ns, stage_tx, stage_lines = pick
     if ns < 2:
         return None
     tiles_hw = -(-H // 16) * -(-W // 8)
@@ -66,8 +84,10 @@ def plan(cin, cout, k, B, D, H, W):
     S = min(max(1, NUM_SMS // jobs), B * D * tiles_hw)
     # every job stages each voxel tile whose input depth slice lies inside the volume, in 16 / ts stages
     valid_tiles = sum(B * max(0, min(D, D - (zd - kd // 2)) - max(0, -(zd - kd // 2))) * tiles_hw for zd in range(kd))
-    staged = -(-cout // MT) * (cin // ntc) * ngroups * valid_tiles * (16 // ts) * stage_tx
-    return dict(jobs=jobs, S=S, ctas=jobs * S, NS=ns, staging="half" if ts == 8 else "whole", staged=staged)
+    stages = -(-cout // MT) * (cin // ntc) * ngroups * valid_tiles * (16 // ts)
+    image = "%s/%s" % ("p8" if x_ch == 8 else "r%d" % x_ch, "p8" if dy_ch == 8 else "r%d" % dy_ch)
+    return dict(jobs=jobs, S=S, ctas=jobs * S, NS=ns, staging="half" if ts == 8 else "whole", image=image,
+                staged=stages * stage_tx, lines=stages * stage_lines)
 
 
 def record_calls(workload):
@@ -186,13 +206,16 @@ def main():
     total_us = sum(r["us"] * r["calls"] for r in rows)
     total_flop = sum(r["flop"] * r["calls"] for r in rows)
     print("workload %s on %s, power limit %s" % (args.workload, name, power))
-    hdr = "%-28s %-7s %-6s %5s %5s %3s %5s %2s %-5s %9s %9s %8s" % ("layer", "x ld+c0", "input", "calls", "jobs", "S", "CTAs",
-                                                                     "NS", "tile", "MB staged", "us", "TFLOP/s")
+    hdr = "%-28s %-7s %-6s %5s %5s %3s %5s %2s %-5s %-7s %9s %8s %9s %8s %9s" % (
+        "layer", "x ld+c0", "input", "calls", "jobs", "S", "CTAs", "NS", "tile", "x/dy", "MB staged", "M lines", "us", "TFLOP/s",
+        "GB/s/CTA")
     print(hdr)
     for r in rows:
-        print("%-28s %-7s %-6s %5d %5s %3s %5s %2s %-5s %9s %9.1f %8.1f" % (
+        per_cta = "%.1f" % (r["staged"] / r["us"] / 1e3 / r["ctas"]) if "staged" in r else "-"
+        print("%-28s %-7s %-6s %5d %5s %3s %5s %2s %-5s %-7s %9s %8s %9.1f %8.1f %9s" % (
             r["shape"], r["x_layout"], r["xform"], r["calls"], r.get("jobs", "-"), r.get("S", "-"), r.get("ctas", "-"), r.get("NS", "-"),
-            r.get("staging", "-"), "%.1f" % (r["staged"] / 1e6) if "staged" in r else "-", r["us"], r["tflops"]))
+            r.get("staging", "-"), r.get("image", "-"), "%.1f" % (r["staged"] / 1e6) if "staged" in r else "-",
+            "%.2f" % (r["lines"] / 1e6) if "lines" in r else "-", r["us"], r["tflops"], per_cta))
     print("per step: %d calls, %.3f ms, %.1f GFLOP, %.1f TFLOP/s (FLOP-weighted)" % (
         sum(r["calls"] for r in rows), total_us / 1e3, total_flop / 1e9, total_flop / total_us / 1e6))
     if args.json:
