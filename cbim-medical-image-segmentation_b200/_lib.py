@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libb200seg.so")
 
 F32, F16 = 0, 1
-ALGO_AUTO, ALGO_DIRECT, ALGO_TC = 0, 1, 2
+ALGO_AUTO, ALGO_DIRECT, ALGO_TC, ALGO_TC_TF32 = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LRELU = 0, 1, 2
 
 P = c_void_p
@@ -35,6 +35,7 @@ _PROTOS = {
     "b200seg_pack_tile_ci": [I],
     "b200seg_pack_weights_multi": [P, P, I, P],
     "b200seg_conv3d_algo": [I, I, I, I, I, I, I],
+    "b200seg_conv3d_algo_tf32": [I, I, I, I, I, I],
     "b200seg_conv3d_fwd": [P, I, I, P, F, I, P, P, P, I, I, P, I, I, P, P, I, I, P, F, I,
                            I, I, I, I, I, I, I, I, I, I, I, P],
     "b200seg_conv3d_wgrad_workspace": [I, I, I, I, I, I, I, I, I, I, I, I, I, I, I, I, I],

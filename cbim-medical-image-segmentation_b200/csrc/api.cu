@@ -42,8 +42,22 @@ extern "C" int b200seg_check_device(void) {
 extern "C" int b200seg_conv3d_algo(int Cin, int Cout, int kd, int kh, int kw, int dtype, int B) {
   // the same batch limits as conv3d_fwd_tc_supported, so every shape routed here runs on the tensor cores with or
   // without fused statistics / dgrad mode
-  if (conv3d_tc_shape_ok(Cin, Cout, kd, kh, kw, dtype) && B * Cin <= 4096 && B * Cout <= 8192) return B200SEG_ALGO_TC;
+  if (dtype == B200SEG_F16 && conv3d_tc_shape_ok(Cin, Cout, kd, kh, kw, dtype) && B * Cin <= 4096 && B * Cout <= 8192)
+    return B200SEG_ALGO_TC;
   return B200SEG_ALGO_DIRECT;
+}
+
+// The fp32 shapes the tensor-core kernel runs on TF32 operands: the kernel-size and batch limits of the fp16 rule, with
+// the TF32 channel table (Cin a multiple of 8, Cout of 16).  The caller decides whether TF32 is wanted at all.
+extern "C" int b200seg_conv3d_algo_tf32(int Cin, int Cout, int kd, int kh, int kw, int B) {
+  if (conv3d_tc_shape_ok(Cin, Cout, kd, kh, kw, B200SEG_F32) && B * Cin <= 4096 && B * Cout <= 8192) return B200SEG_ALGO_TC_TF32;
+  return B200SEG_ALGO_DIRECT;
+}
+
+// TC runs fp16 operands and TC_TF32 fp32 storage on TF32 operands; any other pairing is a caller error
+static int fwd_tc(const ConvArgs& a, int dtype, int algo, cudaStream_t st) {
+  if ((algo == B200SEG_ALGO_TC) != (dtype == B200SEG_F16)) return B200SEG_EUNSUPPORTED;
+  return conv3d_fwd_tc(a, dtype, st);
 }
 
 extern "C" int b200seg_conv3d_fwd(const void* x, int x_ld, int x_coff, const double* x_stats, float eps, int act,
@@ -61,7 +75,7 @@ extern "C" int b200seg_conv3d_fwd(const void* x, int x_ld, int x_coff, const dou
              dgrad_x, dx_ld, dx_coff, dgrad_stats, dgrad_eps, dgrad_act, B, D, H, W, Cin, Cout, kd, kh, kw};
   cudaStream_t st = as_stream(stream);
   // the packed-weight layout differs per algorithm, so the caller must name one (b200seg_conv3d_algo)
-  if (algo == B200SEG_ALGO_TC) return conv3d_fwd_tc(a, dtype, st);
+  if (algo == B200SEG_ALGO_TC || algo == B200SEG_ALGO_TC_TF32) return fwd_tc(a, dtype, algo, st);
   if (algo != B200SEG_ALGO_DIRECT) return B200SEG_EINVAL;
   {
     const int rc = conv3d_fwd_small(a, dtype, st);      // HBM-bound special cases (stem, classifier head)
@@ -82,7 +96,7 @@ extern "C" int b200seg_conv3d_fwd_pc(const void* x, int x_ld, int x_coff, const 
   ConvArgs a{x, x_ld, x_coff, nullptr, 0.f, act, w_packed, bias, residual, r_ld, r_coff, y, y_ld, y_coff, y_stats,
              nullptr, 0, 0, nullptr, 0.f, 0, B, D, H, W, Cin, Cout, kd, kh, kw, x_affine, 1};
   cudaStream_t st = as_stream(stream);
-  if (algo == B200SEG_ALGO_TC) return conv3d_fwd_tc(a, dtype, st);
+  if (algo == B200SEG_ALGO_TC || algo == B200SEG_ALGO_TC_TF32) return fwd_tc(a, dtype, algo, st);
   if (algo != B200SEG_ALGO_DIRECT) return B200SEG_EINVAL;
   {
     const int rc = conv3d_fwd_small(a, dtype, st);

@@ -61,4 +61,11 @@ __host__ __device__ static inline int tc_pick_kc(int Cin) {
     if (Cin % kc == 0) return kc;
   return 0;
 }
+// TF32 K chunk: largest multiple of 8 dividing Cin, <= 32 — the same 16..128 bytes of channels per voxel as tc_pick_kc.
+__host__ __device__ static inline int tc_pick_kc_tf32(int Cin) {
+  if (Cin % 8) return 0;
+  for (int kc = 32; kc >= 8; kc -= 8)
+    if (Cin % kc == 0) return kc;
+  return 0;
+}
 bool conv3d_tc_shape_ok(int Cin, int Cout, int kd, int kh, int kw, int dtype);

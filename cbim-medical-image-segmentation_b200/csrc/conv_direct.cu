@@ -8,6 +8,7 @@
 // unet.py:47 (outc); autograd of the same (train_ddp.py:193/208).
 #include "common.cuh"
 #include "conv_args.h"
+#include "tc_common.cuh"
 
 namespace {
 
@@ -238,38 +239,44 @@ conv_wgrad_direct_kernel(WgradArgs a) {
     atomicAdd(&a.dbias[co0 + threadIdx.x], bacc);
 }
 
-// packed position of element i of a [Cout][Cin][taps] fp32 parameter (see b200seg_pack_weight)
+// packed position of element i of a [Cout][Cin][taps] fp32 parameter (see b200seg_pack_weight).  layout: 0 = DIRECT,
+// 1 = TC (16-byte planes of 8 fp16 channels), 2 = TC_TF32 (16-byte planes of 4 fp32 channels)
 __device__ __forceinline__ int64_t pack_index(int64_t i, int Cout, int Cin, int taps, int transpose_flip, int co_off,
-                                              int co_total, int layout_tc) {
+                                              int co_total, int layout) {
   // virtual packed tensor [taps][R][Cc]: fwd: R = co_total rows (cout), Cc = Cin cols; dgrad operand: R = Cin, Cc = co_total
   const int R = transpose_flip ? Cin : co_total, Cc = transpose_flip ? co_total : Cin;
   const int tap = (int)(i % taps); const int64_t t = i / taps; const int ci = (int)(t % Cin); const int co = (int)(t / Cin);
   const int tp = transpose_flip ? taps - 1 - tap : tap;
   const int row = transpose_flip ? ci : co_off + co;
   const int col = transpose_flip ? co_off + co : ci;
-  if (!layout_tc) return ((int64_t)tp * R + row) * Cc + col;
-  const int NT = tc_pick_nt(R), KC = tc_pick_kc(Cc), NKC = Cc / KC;
-  const int ntile = row / NT, nn = row % NT, kc = col / KC, kk = col % KC, k8 = kk >> 3, e = kk & 7;
-  return ((((int64_t)(ntile * taps + tp) * NKC + kc) * (KC / 8) + k8) * NT + nn) * 8 + e;
+  if (!layout) return ((int64_t)tp * R + row) * Cc + col;
+  const int epp = layout == 2 ? 4 : 8;
+  const int NT = tc_pick_nt(R), KC = layout == 2 ? tc_pick_kc_tf32(Cc) : tc_pick_kc(Cc), NKC = Cc / KC;
+  const int ntile = row / NT, nn = row % NT, kc = col / KC, kk = col % KC, kp = kk / epp, e = kk % epp;
+  return ((((int64_t)(ntile * taps + tp) * NKC + kc) * (KC / epp) + kp) * NT + nn) * epp + e;
 }
+
+// the value stored for weight v: TF32 operands are rounded once here (cvt.rna), so the tensor core sees exact TF32
+__device__ __forceinline__ float pack_value(float v, int layout) { return layout == 2 ? tc::round_tf32(v) : v; }
 
 template <typename T>
 __global__ void pack_weight_kernel(const float* __restrict__ w, int Cout, int Cin, int taps, T* __restrict__ wp,
-                                   int transpose_flip, int co_off, int co_total, int layout_tc) {
+                                   int transpose_flip, int co_off, int co_total, int layout) {
   int64_t n = (int64_t)Cout * Cin * taps;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    Elem<T>::st(wp + pack_index(i, Cout, Cin, taps, transpose_flip, co_off, co_total, layout_tc), w[i]);
+    Elem<T>::st(wp + pack_index(i, Cout, Cin, taps, transpose_flip, co_off, co_total, layout), pack_value(w[i], layout));
 }
 
 // Multi-tensor variant: every conv weight of a model is re-packed by ONE launch per forward (the per-weight
 // launches were ~90 x 12 us per step).  jobs[j] = {w, out, Cout, Cin, taps, dtype, transpose_flip, co_off, co_total,
-// layout_tc}; one block per chunk.  chunks[c] = {job, code}:
+// layout (0 / 1 / 2, as pack_index)}; one block per chunk.  chunks[c] = {job, code}:
 //   code >= 0 : ELEMENT chunk — kPackChunk consecutive source elements from `code`, each written to its packed
 //               position (2-byte scattered stores: 580 us per forward for the 40 M-parameter ResUNet, 10x the HBM time);
 //   code <  0 : TILE chunk (Cout, Cin multiples of 8) — -(code+1) = co0 * 65536 + ci0: eight output channels x up to
 //               pack_tile_ci(taps) input channels x all taps are staged through shared memory (coalesced row reads) and
 //               written as 16-byte groups of the packed image's contiguous 8-element runs (8 consecutive ci of one
-//               (co, tap) in the forward image, 8 consecutive co of one (ci, tap) in the flipped-transposed one).
+//               (co, tap) in the forward image, 8 consecutive co of one (ci, tap) in the flipped-transposed one; in
+//               the TC_TF32 image such a run is two 4-element planes, stored as two 16-byte groups).
 constexpr int kPackChunk = 4096;
 __host__ __device__ inline int pack_tile_ci(int taps) {       // input channels per tile: largest multiple of 8 with 8*ci*taps <= kPackChunk
   const int c = kPackChunk / (8 * taps) / 8 * 8;
@@ -278,7 +285,7 @@ __host__ __device__ inline int pack_tile_ci(int taps) {       // input channels 
 
 template <typename T>
 __device__ __forceinline__ void pack_tile(const float* __restrict__ w, T* __restrict__ o, int Cout, int Cin, int taps, int tf, int co_off,
-                                          int co_total, int tc, int co0, int ci0, float* tile) {
+                                          int co_total, int layout, int co0, int ci0, float* tile) {
   const int cit = min(pack_tile_ci(taps), Cin - ci0), seg = cit * taps;
   for (int idx = threadIdx.x; idx < 8 * seg; idx += 256) {
     const int r = idx / seg, k = idx - r * seg;
@@ -299,7 +306,17 @@ __device__ __forceinline__ void pack_tile(const float* __restrict__ w, T* __rest
       for (int e = 0; e < 8; ++e) v[e] = tile[e * seg + ci * taps + tap];
       first = ((int64_t)co0 * Cin + ci0 + ci) * taps + tap;
     }
-    st8<T>(o + pack_index(first, Cout, Cin, taps, tf, co_off, co_total, tc), v);
+    if constexpr (sizeof(T) == 4) {
+      if (layout == 2) {
+        const int64_t step = 4 * (tf ? (int64_t)Cin * taps : (int64_t)taps);   // source distance of the run's 5th element
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<float4*>(o + pack_index(first + h * step, Cout, Cin, taps, tf, co_off, co_total, layout)) =
+              make_float4(pack_value(v[4 * h], 2), pack_value(v[4 * h + 1], 2), pack_value(v[4 * h + 2], 2), pack_value(v[4 * h + 3], 2));
+        continue;
+      }
+    }
+    st8<T>(o + pack_index(first, Cout, Cin, taps, tf, co_off, co_total, layout), v);
   }
 }
 
@@ -309,22 +326,22 @@ __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const int64_t* 
   const int64_t* j = jobs + 10 * c[0];
   const float* w = reinterpret_cast<const float*>(j[0]);
   const int Cout = (int)j[2], Cin = (int)j[3], taps = (int)j[4], dtype = (int)j[5], tf = (int)j[6], co_off = (int)j[7],
-            co_total = (int)j[8], tc = (int)j[9];
+            co_total = (int)j[8], layout = (int)j[9];
   if (c[1] < 0) {
     const int64_t code = -(c[1] + 1);
     const int co0 = (int)(code >> 16), ci0 = (int)(code & 65535);
-    if (dtype == B200SEG_F16) pack_tile<__half>(w, reinterpret_cast<__half*>(j[1]), Cout, Cin, taps, tf, co_off, co_total, tc, co0, ci0, tile);
-    else pack_tile<float>(w, reinterpret_cast<float*>(j[1]), Cout, Cin, taps, tf, co_off, co_total, tc, co0, ci0, tile);
+    if (dtype == B200SEG_F16) pack_tile<__half>(w, reinterpret_cast<__half*>(j[1]), Cout, Cin, taps, tf, co_off, co_total, layout, co0, ci0, tile);
+    else pack_tile<float>(w, reinterpret_cast<float*>(j[1]), Cout, Cin, taps, tf, co_off, co_total, layout, co0, ci0, tile);
     return;
   }
   const int64_t n = (int64_t)Cout * Cin * taps, i0 = c[1];
   const int64_t i1 = i0 + kPackChunk < n ? i0 + kPackChunk : n;
   if (dtype == B200SEG_F16) {
     __half* o = reinterpret_cast<__half*>(j[1]);
-    for (int64_t i = i0 + threadIdx.x; i < i1; i += 256) o[pack_index(i, Cout, Cin, taps, tf, co_off, co_total, tc)] = __float2half_rn(w[i]);
+    for (int64_t i = i0 + threadIdx.x; i < i1; i += 256) o[pack_index(i, Cout, Cin, taps, tf, co_off, co_total, layout)] = __float2half_rn(w[i]);
   } else {
     float* o = reinterpret_cast<float*>(j[1]);
-    for (int64_t i = i0 + threadIdx.x; i < i1; i += 256) o[pack_index(i, Cout, Cin, taps, tf, co_off, co_total, tc)] = w[i];
+    for (int64_t i = i0 + threadIdx.x; i < i1; i += 256) o[pack_index(i, Cout, Cin, taps, tf, co_off, co_total, layout)] = pack_value(w[i], layout);
   }
 }
 
@@ -376,11 +393,12 @@ int conv3d_wgrad_direct(const WgradArgs& a_in, int dtype, cudaStream_t st) {
 extern "C" int b200seg_pack_weight(const float* w, int Cout, int Cin, int taps, void* w_packed, int dtype,
                                    int transpose_flip, int co_off, int co_total, int layout, void* stream) {
   if (!w || !w_packed || Cout <= 0 || Cin <= 0 || taps <= 0 || co_off < 0 || co_off + Cout > co_total) return B200SEG_EINVAL;
-  if (layout != B200SEG_ALGO_DIRECT && layout != B200SEG_ALGO_TC) return B200SEG_EINVAL;
-  const int tc = layout == B200SEG_ALGO_TC;
+  if (layout != B200SEG_ALGO_DIRECT && layout != B200SEG_ALGO_TC && layout != B200SEG_ALGO_TC_TF32) return B200SEG_EINVAL;
+  const int tc = layout == B200SEG_ALGO_TC ? 1 : layout == B200SEG_ALGO_TC_TF32 ? 2 : 0;     // pack_index layout code
   if (tc) {
     const int R = transpose_flip ? Cin : co_total, Cc = transpose_flip ? co_total : Cin;
-    if (!tc_pick_nt(R) || !tc_pick_kc(Cc) || dtype != B200SEG_F16) return B200SEG_EUNSUPPORTED;
+    if (!tc_pick_nt(R) || !(tc == 1 ? tc_pick_kc(Cc) : tc_pick_kc_tf32(Cc)) || dtype != (tc == 1 ? B200SEG_F16 : B200SEG_F32))
+      return B200SEG_EUNSUPPORTED;
   }
   cudaStream_t st = as_stream(stream);
   int64_t n = (int64_t)Cout * Cin * taps;

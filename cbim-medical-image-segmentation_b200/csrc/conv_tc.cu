@@ -1,25 +1,29 @@
-// conv_tc.cu — conv3d forward / data-gradient as a wgmma implicit GEMM (sm_90a), fp16 operands, fp32 accumulation
-// in registers.  Replaces cuDNN fprop/dgrad behind nn.Conv3d (conv_layers.py:29-38) and fuses the surrounding
-// InstanceNorm+ReLU (conv_layers.py:40-43), residual add (:92) and the next layer's InstanceNorm reduction.
+// conv_tc.cu — conv3d forward / data-gradient as a wgmma implicit GEMM (sm_90a), fp16 or TF32 operands, fp32
+// accumulation in registers.  Replaces cuDNN fprop/dgrad behind nn.Conv3d (conv_layers.py:29-38) and fuses the
+// surrounding InstanceNorm+ReLU (conv_layers.py:40-43), residual add (:92) and the next layer's InstanceNorm reduction.
 //
 // GEMM view (per CTA tile):  D[128 voxels][NT cout] += A[128 voxels][KC cin] * B[KC cin][NT cout]
 // for every filter tap and every KC-chunk of Cin.
 //   * M tile  = 16(h) x 8(w) output voxels of one depth slice; GEMM row r = hl*8 + wl.
 //   * A operand = a HALO tile (16+kh-1)x(8+kw-1) voxels x KC channels of ONE input depth slice, staged
-//     once in shared memory as [KC/8][halo voxel][8 ch] (K-major, no-swizzle core matrices:
-//     8 consecutive w-voxels x 16 B).  Every (kh,kw) tap reads the SAME staged tile through a shifted
+//     once in shared memory as [KC/8][halo voxel][8 ch] (fp32: [KC/4][halo voxel][4 ch]) (K-major, no-swizzle core
+//     matrices: 8 consecutive w-voxels x 16 B).  Every (kh,kw) tap reads the SAME staged tile through a shifted
 //     matrix descriptor (start += (zh*HALO_W + zw)*16 B, SBO = HALO_W*16 B) — im2col is never formed.
 //   * Staging: raw inputs (every data-gradient launch) arrive as one tensor-TMA box per stage; inputs that need
 //     InstanceNorm / activation are copied by the loader warps (TMA box or 16-byte cp.async, up to three stages
 //     ahead), normalised + activated IN PLACE in shared memory and then published to the MMA warpgroups.  The
 //     normalised activation tensor never exists in HBM.
 //   * B operand = weights pre-packed on device into the exact shared-memory image per (ntile,tap,kchunk)
-//     ([KC/8][NT][8] fp16): resident for the CTA's lifetime when the layer's weights fit (<=112 KB), else streamed
-//     by 1-D bulk TMA (cp.async.bulk) through an mbarrier ring.
+//     ([KC/8][NT][8] fp16, [KC/4][NT][4] fp32): resident for the CTA's lifetime when the layer's weights fit
+//     (<=112 KB), else streamed by 1-D bulk TMA (cp.async.bulk) through an mbarrier ring.
 //   * D lives in the registers of two consumer warpgroups (64 rows each, wgmma m64 x NT x 16), which also run the
-//     epilogue: bias / residual / dgrad ReLU-mask, fp16 store, InstanceNorm sums of the stored tile.  The epilogue's
-//     side operand (residual, or the pre-norm input of the dgrad mask) is one tensor-TMA box per tile in shared memory,
-//     issued a tile or more ahead, so no epilogue waits on a global load.
+//     epilogue: bias / residual / dgrad ReLU-mask, fp16 (or fp32) store, InstanceNorm sums of the stored tile.  The
+//     epilogue's side operand (residual, or the pre-norm input of the dgrad mask) is one tensor-TMA box per tile in
+//     shared memory, issued a tile or more ahead, so no epilogue waits on a global load.
+// TF32 (fp32 storage, operand type T = float): every byte of the geometry is the fp16 kernel's.  A 16-byte channel plane
+// holds 4 channels instead of 8, KC is at most 32 (tc_pick_kc_tf32) and a K step is k8 instead of k16, so a stage holds
+// the same bytes and takes the same KSTEPS wgmma instructions per tap.  Weights and loader-transformed inputs are
+// rounded to TF32 (cvt.rna) by the library; raw TMA-staged inputs reach the tensor core unchanged.
 // Warp roles (640 threads = 5 warpgroups, 1 CTA/SM, persistent over tiles; `setmaxnreg` moves registers from the
 // loader / weight warpgroups to the two consumer warpgroups, whose accumulators need them):
 //   warps 0-7  MMA + epilogue (warpgroup g = GEMM rows 64g .. 64g+63)
@@ -53,7 +57,7 @@ static_assert(2 * 128 * kRegsConsumer + 2 * 128 * kRegsLoad + 128 * kRegsWgt <= 
 
 struct TcParams {
   ConvArgs a;
-  const void* wimg;        // weight image [ntile][tap][kchunk][KC/8][NT][8]
+  const void* wimg;        // weight image [ntile][tap][kchunk][KC/EPP][NT][EPP], EPP = channels per 16-byte plane
   int KC, NKC, NT, NTILES;
   int HALO_H, HALO_W, nvox_h, plane_stride;   // plane_stride in bytes (odd multiple of 16)
   int a_stage_bytes, b_stage_bytes, SA, SB;
@@ -61,11 +65,11 @@ struct TcParams {
   int w_resident;          // all weights of the layer live in shared memory for the CTA's lifetime (no B ring)
   int prefetch;            // A stages the loaders keep in flight (1..3, < SA)
   int use_tma;             // halo tiles are staged by ONE tensor-TMA box per stage (else 16-byte cp.async copies)
-  int SS, side_stage_bytes; // side-operand slots (residual / dgrad_x tile, [NT/8 planes][128 voxels][8 ch]); 0 = none
+  int SS, side_stage_bytes; // side-operand slots (residual / dgrad_x tile, [NT/EPP planes][128 voxels][EPP ch]); 0 = none
   int smem_a_off, smem_b_off, smem_side_off, smem_bar_off, smem_norm_off, smem_gnorm_off;
   int norm_bstride;        // entries per sample in the {scale, shift} table: Cin, or 0 for a per-channel table
-  alignas(64) CUtensorMap tm_x;      // x as {8 ch, w, h, channel plane, b*D + d}
-  alignas(64) CUtensorMap tm_side;   // res or gx (Cout channels), same dims; box {8, TW, TH, NT/8}
+  alignas(64) CUtensorMap tm_x;      // x as {EPP ch, w, h, channel plane, b*D + d}
+  alignas(64) CUtensorMap tm_side;   // res or gx (Cout channels), same dims; box {EPP, TW, TH, NT/EPP}
 };
 
 // barrier block layout (uint64 each): a_full[SA] a_empty[SA] b_full[SB] b_empty[SB] a_land[SA] side_full[SS]
@@ -137,8 +141,8 @@ struct StageCursor {
 
 // ------------------------------------------------------------------ A loaders
 // cp.async (LDGSTS) prefetch of P stages + in-place InstanceNorm/ReLU once a stage has landed.  Each thread owns ONE
-// 8-channel plane and a fixed set of (at most kMaxChunks) halo voxels of it, copies exactly those 16-byte chunks and
-// later transforms exactly those chunks, so no cross-thread synchronisation is needed between copy and transform.
+// 16-byte channel plane and a fixed set of (at most kMaxChunks) halo voxels of it, copies exactly those 16-byte chunks
+// and later transforms exactly those chunks, so no cross-thread synchronisation is needed between copy and transform.
 // Everything that does not depend on the tile (voxel slot, offset from the tile origin, halo row / column) is computed
 // once per thread; per stage the work is one pointer add per chunk, and the bounds tests vanish for interior tiles.
 constexpr int kMaxChunks = 6;
@@ -146,18 +150,27 @@ constexpr int kMaxChunks = 6;
 // 18 x 10 halo voxels over at least 256 / 8 threads per plane
 static_assert(kMaxChunks * (kLoadThreads / (64 / 8)) >= (TH + 2) * (TW + 2), "loader chunk table smaller than the largest halo tile");
 
-template <int P, bool TMA>
+// channels of operand type T in one 16-byte plane (8 fp16, 4 fp32); tc_pick_kc / tc_pick_kc_tf32 both give <= 8 planes
+template <typename T> constexpr int kEpp = 16 / (int)sizeof(T);
+template <typename T, bool RELU>
+__device__ __forceinline__ uint4 norm_act_plane(uint4 raw, const float (&sc)[kEpp<T>], const float (&sf)[kEpp<T>], float slope) {
+  if constexpr (sizeof(T) == 4) return norm_act4<RELU>(raw, sc, sf, slope);
+  else return norm_act8<RELU>(raw, sc, sf, slope);
+}
+
+template <typename T, int P, bool TMA>
 __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, const float2* s_norm, const Bars& bars) {
+  constexpr int EPP = kEpp<T>;
   const ConvArgs& a = p.a;
   const int lt = threadIdx.x - kLoadWarp0 * 32;
-  const int cpv = p.KC / 8;
+  const int cpv = p.KC / EPP;
   const int vstep = kLoadThreads / cpv;
   const bool active = lt < vstep * cpv;
   const int c8 = lt % cpv, v0 = lt / cpv;
   const int ph = a.kh / 2, pw = a.kw / 2;
   const bool xform = (a.x_stats != nullptr) || (a.x_affine != nullptr) || (a.act != 0);
   const int act = a.act;
-  const __half* xbase = reinterpret_cast<const __half*>(a.x);
+  const T* xbase = reinterpret_cast<const T*>(a.x);
   const uint32_t smem_a = smem_u32(smem + p.smem_a_off) + (uint32_t)(c8 * p.plane_stride);
   uint8_t* smem_a_gen = smem + p.smem_a_off + c8 * p.plane_stride;
   // TMA mode: thread 0 stages the halo tile with ONE tensor-TMA box per stage; every thread then transforms exactly
@@ -174,7 +187,7 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
     const bool have = active && v < p.nvox_h;
     const int hh = v / p.HALO_W, ww = v % p.HALO_W;
     if constexpr (TMA) {
-      rel[i] = c8 * p.plane_stride + v * 16;      // byte offset of the chunk inside a stage: plane image [c8][v][8 ch]
+      rel[i] = c8 * p.plane_stride + v * 16;      // byte offset of the chunk inside a stage: plane image [c8][v][EPP ch]
     } else {
       rel[i] = (hh * a.W + ww) * a.x_ld;
     }
@@ -202,7 +215,7 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
     const uint32_t dst = smem_a + (uint32_t)(ri.idx * p.a_stage_bytes) + (uint32_t)v0 * 16u;
     const int hb = ci.ti.hi * TH - ph, wb = ci.ti.wi * TW - pw;
     const bool interior = hb >= 0 && wb >= 0 && hb + p.HALO_H <= a.H && wb + p.HALO_W <= a.W;
-    const __half* xs = xbase + (((int64_t)(ci.ti.b * a.D + ci.din) * a.H + hb) * a.W + wb) * a.x_ld + a.x_coff + ci.kc * p.KC + c8 * 8;
+    const T* xs = xbase + (((int64_t)(ci.ti.b * a.D + ci.din) * a.H + hb) * a.W + wb) * a.x_ld + a.x_coff + ci.kc * p.KC + c8 * EPP;
 #pragma unroll
     for (int i = 0; i < kMaxChunks; ++i) {
       if (i < nch && hw[i] != 0xffffffffu) {
@@ -216,7 +229,7 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
 
   const float slope = act_slope(act);
   const bool relu = act == B200SEG_ACT_RELU;
-  float sc[8], sf[8];                              // x*sc + sf: (x - mean) * rstd, or the per-channel affine transform
+  float sc[EPP], sf[EPP];                          // x*sc + sf: (x - mean) * rstd, or the per-channel affine transform
   int norm_key = -1;                               // (b, kc) the constants belong to
 #pragma unroll
   for (int i = 0; i < P; ++i) { if (ci.valid(tw)) issue(); if constexpr (!TMA) cp_async_commit(); }
@@ -228,8 +241,8 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
       if (key != norm_key) {
         norm_key = key;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float2 st = s_norm[cd.ti.b * p.norm_bstride + cd.kc * p.KC + c8 * 8 + j];
+        for (int j = 0; j < EPP; ++j) {
+          const float2 st = s_norm[cd.ti.b * p.norm_bstride + cd.kc * p.KC + c8 * EPP + j];
           sc[j] = st.x; sf[j] = st.y;
         }
       }
@@ -254,10 +267,10 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
         if constexpr (TMA) {      // one branch per batch: the three chunks' dependency chains interleave
           if (relu) {
 #pragma unroll
-            for (int u = 0; u < 3; ++u) raw[u] = norm_act8<true>(raw[u], sc, sf, slope);
+            for (int u = 0; u < 3; ++u) raw[u] = norm_act_plane<T, true>(raw[u], sc, sf, slope);
           } else {
 #pragma unroll
-            for (int u = 0; u < 3; ++u) raw[u] = norm_act8<false>(raw[u], sc, sf, slope);
+            for (int u = 0; u < 3; ++u) raw[u] = norm_act_plane<T, false>(raw[u], sc, sf, slope);
           }
 #pragma unroll
           for (int u = 0; u < 3; ++u)
@@ -266,7 +279,7 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
 #pragma unroll
           for (int u = 0; u < 3; ++u) {
             if (!ok[u]) continue;
-            raw[u] = relu ? norm_act8<true>(raw[u], sc, sf, slope) : norm_act8<false>(raw[u], sc, sf, slope);
+            raw[u] = relu ? norm_act_plane<T, true>(raw[u], sc, sf, slope) : norm_act_plane<T, false>(raw[u], sc, sf, slope);
             *reinterpret_cast<uint4*>(chunk(i0 + u)) = raw[u];
           }
         }
@@ -282,21 +295,23 @@ __device__ __forceinline__ void loader_role(const TcParams& p, uint8_t* smem, co
 }
 
 // ---- TMA staging of RAW inputs (every data-gradient launch): one elected loader thread issues ONE tensor-TMA box
-// {8 ch, HALO_W, HALO_H, KC/8 planes} per stage — the TMA unit writes the [plane][halo voxel][8 ch] image and zero-fills
-// conv padding / ragged tiles — and the MMA warpgroups consume the stage straight off the TMA's transaction barrier: no
+// {EPP ch, HALO_W, HALO_H, KC/EPP planes} per stage — the TMA unit writes the [plane][halo voxel][EPP ch] image and
+// zero-fills conv padding / ragged tiles — and the MMA warpgroups consume the stage straight off the TMA's transaction barrier: no
 // loader instruction touches the data.  (Inputs that need InstanceNorm / activation go through loader_role<P>, whose TMA
 // mode lands the same box and then transforms it in place with the cp.async path's per-thread chunk table.)
+template <typename T>
 __device__ __forceinline__ void loader_role_tma(const TcParams& p, uint8_t* smem, const Bars& bars) {
+  constexpr int EPP = kEpp<T>;
   const ConvArgs& a = p.a;
   const int lt = threadIdx.x - kLoadWarp0 * 32;
   const int ph = a.kh / 2, pw = a.kw / 2;
   const uint32_t smem_a = smem_u32(smem + p.smem_a_off);
   TileWalk tw; tw.init(p);
-  const uint32_t stage_tx = (uint32_t)((p.KC / 8) * p.nvox_h * 16);
+  const uint32_t stage_tx = (uint32_t)((p.KC / EPP) * p.nvox_h * 16);
   auto issue = [&](const StageCursor& c, int slot) {
     mbar_arrive_expect_tx(bars.a_land(slot), stage_tx);
     tma_load_5d(smem_a + (uint32_t)(slot * p.a_stage_bytes), &p.tm_x, bars.a_land(slot), 0, c.ti.wi * TW - pw, c.ti.hi * TH - ph,
-                  c.kc * (p.KC / 8), c.ti.b * a.D + c.din);
+                  c.kc * (p.KC / EPP), c.ti.b * a.D + c.din);
   };
   if (lt == 0) {
     StageCursor c; c.init(tw, p);
@@ -319,10 +334,13 @@ __device__ __forceinline__ void loader_role_tma(const TcParams& p, uint8_t* smem
 // and kept in registers (lane l keeps the groups j with j % 8 == l / 4) while consecutive tiles share a (batch, N tile);
 // then each warp adds them to y_stats with one fp64 atomic per value.  Every addition before the atomic happens in a
 // fixed order; the order of the fp64 atomics can move only the last fp64 bits of the statistics.
-// KSTEPS = KC / 16 is a template argument so that a tap's group is straight-line code: with a run-time trip count the
-// unrolled loop and its remainder made ptxas move accumulators between the MMAs and serialise them (C7519).
-template <int NT, int KSTEPS>
+// KSTEPS = KC / 16 (fp16) or KC / 8 (TF32) is a template argument so that a tap's group is straight-line code: with a
+// run-time trip count the unrolled loop and its remainder made ptxas move accumulators between the MMAs and serialise
+// them (C7519).
+template <typename T, int NT, int KSTEPS>
 __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid, uint8_t* smem, const Bars& bars, const float2* s_gnorm) {
+  constexpr bool F32 = sizeof(T) == 4;
+  constexpr int EPP = kEpp<T>;
   const ConvArgs& a = p.a;
   // A stage ready: published by the loaders, or (raw input staged by TMA) the TMA's own transaction barrier
   const uint32_t a_ready0 = (p.use_tma && !(a.x_stats || a.x_affine || a.act)) ? bars.a_land(0) : bars.a_full(0);
@@ -403,7 +421,8 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
             wgmma_fence();
 #pragma unroll
             for (int j = 0; j < KSTEPS; ++j)
-              Wgmma<NT, 0, 0>::mma(acc, da + (uint64_t)((uint32_t)j * a_kstep), db + (uint64_t)((uint32_t)j * b_kstep), accumulate | (uint32_t)(j > 0));
+              if constexpr (F32) WgmmaTf32<NT>::mma(acc, da + (uint64_t)((uint32_t)j * a_kstep), db + (uint64_t)((uint32_t)j * b_kstep), accumulate | (uint32_t)(j > 0));
+              else Wgmma<NT, 0, 0>::mma(acc, da + (uint64_t)((uint32_t)j * a_kstep), db + (uint64_t)((uint32_t)j * b_kstep), accumulate | (uint32_t)(j > 0));
             accumulate = 1;
             wgmma_commit();
             wgmma_wait<1>();                       // the previous group has retired: its slots are free
@@ -420,20 +439,23 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
     wgmma_fence_operands(acc);
     release();
 
-    // ---- epilogue: bias / residual / dgrad mask, fp16 rounding and store, InstanceNorm sums
+    // ---- epilogue: bias / residual / dgrad mask, fp16 rounding (none in fp32) and store, InstanceNorm sums
     const int co_base = tc.ntile * NT;
-    __half* yp[2];
+    T* yp[2];
     bool valid[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int h = tc.h0 + hl0 + i, w = tc.w0 + wl;
       valid[i] = h < a.H && w < a.W;
       const int64_t vox = ((int64_t)(tc.b * a.D + tc.d) * a.H + (valid[i] ? h : 0)) * a.W + (valid[i] ? w : 0);
-      yp[i] = reinterpret_cast<__half*>(a.y) + vox * a.y_ld + a.y_coff + co_base;
+      yp[i] = reinterpret_cast<T*>(a.y) + vox * a.y_ld + a.y_coff + co_base;
     }
-    // side tile [NT/8 planes][128 rows][8 ch]: rows r0, r0 + 8 of plane j; the 8 lanes sharing a plane read 128
-    // consecutive bytes
-    const uint8_t* side = smem + p.smem_side_off + rs.idx * p.side_stage_bytes + r0 * 16 + 4 * (lane & 3);
+    // side tile [NT/EPP planes][128 rows][EPP ch]: rows r0, r0 + 8 of column group j = planes j*8/EPP ..; the lanes
+    // sharing a plane read 128 consecutive bytes
+    const int cl = 2 * (lane & 3);                                     // column of the pair inside its group of 8
+    const uint8_t* side = smem + p.smem_side_off + rs.idx * p.side_stage_bytes + r0 * 16 + (cl / EPP) * (TH * TW * 16) +
+                          (cl % EPP) * (int)sizeof(T);
+    auto rnd = [](float v) { if constexpr (F32) return v; else return __half2float(__float2half_rn(v)); };
     if (has_side) mbar_wait(bars.side_full(rs.idx), rs.phase);
     const float2* gn = s_gnorm + tc.b * a.Cout + co_base;
     if (want_stats && tc.b * p.NTILES + tc.ntile != stat_key) { flush(); stat_key = tc.b * p.NTILES + tc.ntile; }
@@ -448,19 +470,24 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
         if (!valid[i]) continue;                 // rows outside the volume: nothing stored, nothing counted
         float v0 = acc[4 * j + 2 * i] + bv.x, v1 = acc[4 * j + 2 * i + 1] + bv.y;
         float2 sv = make_float2(0.f, 0.f);
-        if (has_side) sv = __half22float2(*reinterpret_cast<const __half2*>(side + j * (TH * TW * 16) + i * 128));
+        if (has_side) {
+          const uint8_t* sp = side + j * (8 / EPP) * (TH * TW * 16) + i * 128;
+          if constexpr (F32) sv = *reinterpret_cast<const float2*>(sp);
+          else sv = __half22float2(*reinterpret_cast<const __half2*>(sp));
+        }
         if (dgrad) {
           const float4 mr = *reinterpret_cast<const float4*>(gn + c);      // {mean, rstd} of two channels
           const float h0 = (sv.x - mr.x) * mr.y, h1 = (sv.y - mr.z) * mr.w;
-          v0 = __half2float(__float2half_rn(v0 * act_grad_s(h0, gslope)));
-          v1 = __half2float(__float2half_rn(v1 * act_grad_s(h1, gslope)));
+          v0 = rnd(v0 * act_grad_s(h0, gslope));
+          v1 = rnd(v1 * act_grad_s(h1, gslope));
           s0 += v0; s1 += v1; q0 = fmaf(v0, h0, q0); q1 = fmaf(v1, h1, q1);
         } else {
-          v0 = __half2float(__float2half_rn(v0)); v1 = __half2float(__float2half_rn(v1));
-          if (has_side) { v0 = __half2float(__float2half_rn(v0 + sv.x)); v1 = __half2float(__float2half_rn(v1 + sv.y)); }
+          v0 = rnd(v0); v1 = rnd(v1);
+          if (has_side) { v0 = rnd(v0 + sv.x); v1 = rnd(v1 + sv.y); }
           s0 += v0; s1 += v1; q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
         }
-        *reinterpret_cast<__half2*>(yp[i] + c) = __floats2half2_rn(v0, v1);
+        if constexpr (F32) *reinterpret_cast<float2*>(yp[i] + c) = make_float2(v0, v1);
+        else *reinterpret_cast<__half2*>(yp[i] + c) = __floats2half2_rn(v0, v1);
       }
       if (want_stats) {
 #pragma unroll
@@ -477,11 +504,9 @@ __device__ __forceinline__ void consumer_role(const TcParams& p, int wg, int tid
 }
 
 // ------------------------------------------------------------------ the kernel
-// One instantiation per (NT, KC / 16) that tc_pick_nt / tc_pick_kc can produce, so each gets its own register
-// allocation instead of sharing the worst case of every tile width.
-template <int NT, int KSTEPS>
-__global__ void __launch_bounds__(kThreads, 1)
-conv_tc_kernel(const __grid_constant__ TcParams p) {
+// The whole kernel for operand type T; conv_tc_kernel (fp16) and conv_tc_kernel_tf32 below are its two entry points.
+template <typename T, int NT, int KSTEPS>
+__device__ __forceinline__ void conv_tc_body(const TcParams& p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const ConvArgs& a = p.a;
   // canonical warp index: the shuffle makes it provably warp-uniform, so the role branches below are uniform branches
@@ -525,10 +550,10 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   if (warp >= kLoadWarp0 && warp < kWgtWarp) {
     // =========================== A LOADERS ===========================
     setmaxnreg_dec<kRegsLoad>();
-    if (p.use_tma && !(a.x_stats || a.x_affine || a.act)) loader_role_tma(p, smem, bars);
-    else if (p.use_tma) loader_role<3, true>(p, smem, s_norm, bars);
-    else if (p.prefetch >= 3) loader_role<3, false>(p, smem, s_norm, bars);
-    else loader_role<1, false>(p, smem, s_norm, bars);
+    if (p.use_tma && !(a.x_stats || a.x_affine || a.act)) loader_role_tma<T>(p, smem, bars);
+    else if (p.use_tma) loader_role<T, 3, true>(p, smem, s_norm, bars);
+    else if (p.prefetch >= 3) loader_role<T, 3, false>(p, smem, s_norm, bars);
+    else loader_role<T, 1, false>(p, smem, s_norm, bars);
   } else if (warp >= kWgtWarp) {
     setmaxnreg_dec<kRegsWgt>();
     if (warp == kWgtWarp && lane == 0) {
@@ -572,7 +597,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
         mbar_wait(bars.side_empty(ring.idx), ring.phase ^ 1);
         mbar_arrive_expect_tx(bars.side_full(ring.idx), (uint32_t)p.side_stage_bytes);
         tma_load_5d(smem_side + (uint32_t)(ring.idx * p.side_stage_bytes), &p.tm_side, bars.side_full(ring.idx), 0, ti.wi * TW,
-                    ti.hi * TH, ti.ntile * (p.NT / 8), ti.b * a.D + ti.d);
+                    ti.hi * TH, ti.ntile * (p.NT / kEpp<T>), ti.b * a.D + ti.d);
         ring.advance();
       }
     }
@@ -580,11 +605,22 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
     // =========================== MMA + EPILOGUE (warps 0-7) ===========================
     setmaxnreg_inc<kRegsConsumer>();
     const int wg = warp >> 2, tid = threadIdx.x & 127;
-    consumer_role<NT, KSTEPS>(p, wg, tid, smem, bars, s_gnorm);
+    consumer_role<T, NT, KSTEPS>(p, wg, tid, smem, bars, s_gnorm);
   }
 }
 
-// KC / 16 for KC in {16, 32, 48, 64} (tc_pick_kc) as a compile-time constant
+// One instantiation per (NT, KSTEPS) that tc_pick_nt / tc_pick_kc (fp16) or tc_pick_kc_tf32 (TF32) can produce, so each
+// gets its own register allocation instead of sharing the worst case of every tile width.
+template <int NT, int KSTEPS>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_tc_kernel(const __grid_constant__ TcParams p) { conv_tc_body<__half, NT, KSTEPS>(p); }
+
+template <int NT, int KSTEPS>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_tc_kernel_tf32(const __grid_constant__ TcParams p) { conv_tc_body<float, NT, KSTEPS>(p); }
+
+// KSTEPS for KC in {16, 32, 48, 64} (fp16, tc_pick_kc) or {8, 16, 24, 32} (TF32, tc_pick_kc_tf32) as a compile-time
+// constant
 template <class F>
 void dispatch_ksteps(int ksteps, F&& f) {
   switch (ksteps) {
@@ -595,32 +631,35 @@ void dispatch_ksteps(int ksteps, F&& f) {
   }
 }
 
-template <int NT, int KSTEPS>
+template <typename T, int NT, int KSTEPS>
 int launch_conv_tc(const TcParams& p, int grid, int smem_bytes, cudaStream_t st) {
+  constexpr auto kernel = sizeof(T) == 4 ? conv_tc_kernel_tf32<NT, KSTEPS> : conv_tc_kernel<NT, KSTEPS>;
   static thread_local bool attr_set = false;
   if (!attr_set) {
-    B200_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT, KSTEPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  conv_tc_kernel<NT, KSTEPS><<<grid, kThreads, smem_bytes, st>>>(p);
-  B200_CHECK_LAUNCH("conv_tc_kernel");
+  kernel<<<grid, kThreads, smem_bytes, st>>>(p);
+  B200_CHECK_LAUNCH(sizeof(T) == 4 ? "conv_tc_kernel_tf32" : "conv_tc_kernel");
   return B200SEG_OK;
 }
 
 }  // namespace
 
+// dtype names the operand type: B200SEG_F16 = fp16 operands, B200SEG_F32 = fp32 storage on TF32 operands
 bool conv3d_tc_shape_ok(int Cin, int Cout, int kd, int kh, int kw, int dtype) {
-  if (dtype != B200SEG_F16) return false;
-  if (tc_pick_nt(Cout) == 0 || tc_pick_kc(Cin) == 0) return false;
+  if (dtype != B200SEG_F16 && dtype != B200SEG_F32) return false;
+  if (tc_pick_nt(Cout) == 0 || (dtype == B200SEG_F16 ? tc_pick_kc(Cin) : tc_pick_kc_tf32(Cin)) == 0) return false;
   if (kh > 3 || kw > 3 || kd > 3 || kd < 1 || kh < 1 || kw < 1) return false;
   return true;
 }
 
 bool conv3d_fwd_tc_supported(const ConvArgs& a, int dtype) {
   if (!conv3d_tc_shape_ok(a.Cin, a.Cout, a.kd, a.kh, a.kw, dtype)) return false;
-  if ((a.x_ld % 8) || (a.x_coff % 8) || (a.y_ld % 8) || (a.y_coff % 8)) return false;
-  if (a.res && ((a.r_ld % 8) || (a.r_coff % 8))) return false;
-  if (a.gx && ((a.gx_ld % 8) || (a.gx_coff % 8))) return false;
+  const int epp = dtype == B200SEG_F16 ? 8 : 4;       // elements per 16 bytes: every row and channel offset is 16-byte aligned
+  if ((a.x_ld % epp) || (a.x_coff % epp) || (a.y_ld % epp) || (a.y_coff % epp)) return false;
+  if (a.res && ((a.r_ld % epp) || (a.r_coff % epp))) return false;
+  if (a.gx && ((a.gx_ld % epp) || (a.gx_coff % epp))) return false;
   if ((reinterpret_cast<uintptr_t>(a.x) | reinterpret_cast<uintptr_t>(a.y) | reinterpret_cast<uintptr_t>(a.w)) & 15) return false;
   // the residual / dgrad_x tile is a tensor-TMA box: 16-byte aligned base
   if ((reinterpret_cast<uintptr_t>(a.res) | reinterpret_cast<uintptr_t>(a.gx)) & 15) return false;
@@ -633,14 +672,17 @@ bool conv3d_fwd_tc_supported(const ConvArgs& a, int dtype) {
   return true;
 }
 
-// `a.w` must be the TC weight IMAGE ([ntile][tap][kchunk][KC/8][NT][8], b200seg_pack_weight layout=TC).
+// `a.w` must be the TC weight IMAGE: [ntile][tap][kchunk][KC/8][NT][8] fp16 (b200seg_pack_weight layout=TC), or
+// [ntile][tap][kchunk][KC/4][NT][4] TF32-rounded fp32 (layout=TC_TF32) when dtype is B200SEG_F32.
 int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
   if (!conv3d_fwd_tc_supported(a, dtype)) return B200SEG_EUNSUPPORTED;
+  const bool f32 = dtype == B200SEG_F32;
+  const int es = f32 ? 4 : 2, epp = 16 / es;          // bytes per element, elements per 16-byte channel plane
   TcParams p;
   memset(&p, 0, sizeof(p));
   p.a = a;
   p.wimg = a.w;
-  p.KC = tc_pick_kc(a.Cin); p.NKC = a.Cin / p.KC;
+  p.KC = f32 ? tc_pick_kc_tf32(a.Cin) : tc_pick_kc(a.Cin); p.NKC = a.Cin / p.KC;
   p.NT = tc_pick_nt(a.Cout); p.NTILES = a.Cout / p.NT;
   p.HALO_H = TH + a.kh - 1; p.HALO_W = TW + a.kw - 1;
   p.nvox_h = p.HALO_H * p.HALO_W;
@@ -651,24 +693,24 @@ int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
   // cp.async copies + transform otherwise.  When the tensor map cannot be built every input takes the cp.async path.
   const bool raw_input = !a.x_stats && !a.x_affine && a.act == 0;
   p.use_tma = ((raw_input || a.Cin <= 64) &&
-               b200seg_make_act_tmap(&p.tm_x, a.x, a.x_ld, a.x_coff, a.Cin, a.B * a.D, a.H, a.W, p.HALO_W, p.HALO_H, p.KC / 8)) ? 1 : 0;
+               b200seg_make_act_tmap(&p.tm_x, a.x, a.x_ld, a.x_coff, a.Cin, a.B * a.D, a.H, a.W, p.HALO_W, p.HALO_H, p.KC / epp, epp, f32)) ? 1 : 0;
   p.plane_stride = p.use_tma ? p.nvox_h * 16 : slots * 16;    // a TMA box is written densely
-  p.a_stage_bytes = (p.KC / 8) * p.plane_stride;
+  p.a_stage_bytes = (p.KC / epp) * p.plane_stride;
   p.a_stage_bytes = (p.a_stage_bytes + 127) / 128 * 128;      // TMA destinations are 128-byte aligned
-  p.b_stage_bytes = p.KC * p.NT * 2;
+  p.b_stage_bytes = p.KC * p.NT * es;
   p.tiles_h = (a.H + TH - 1) / TH; p.tiles_w = (a.W + TW - 1) / TW;
   int64_t nt = (int64_t)a.B * a.D * p.tiles_h * p.tiles_w * p.NTILES;
   if (nt > 0x7fffffff) return B200SEG_EUNSUPPORTED;
   p.n_tiles = (int)nt;
   // The epilogue's side operand (residual, or dgrad_x behind the activation mask) arrives as one tensor-TMA box
-  // {8 ch, TW, TH, NT/8 planes} per tile, zero-filled past the volume edge, in a ring of SS slots.  Narrow tiles
+  // {EPP ch, TW, TH, NT/EPP planes} per tile, zero-filled past the volume edge, in a ring of SS slots.  Narrow tiles
   // (NT <= 64) take only a few hundred clocks of MMAs, so their box is issued two tiles ahead; wider tiles are long
   // enough for one slot.
   if (a.res || a.gx) {
     p.SS = p.NT <= 64 ? 2 : 1;
-    p.side_stage_bytes = TH * TW * p.NT * 2;
-    const bool ok = a.gx ? b200seg_make_act_tmap(&p.tm_side, a.gx, a.gx_ld, a.gx_coff, a.Cout, a.B * a.D, a.H, a.W, TW, TH, p.NT / 8)
-                         : b200seg_make_act_tmap(&p.tm_side, a.res, a.r_ld, a.r_coff, a.Cout, a.B * a.D, a.H, a.W, TW, TH, p.NT / 8);
+    p.side_stage_bytes = TH * TW * p.NT * es;
+    const bool ok = a.gx ? b200seg_make_act_tmap(&p.tm_side, a.gx, a.gx_ld, a.gx_coff, a.Cout, a.B * a.D, a.H, a.W, TW, TH, p.NT / epp, epp, f32)
+                         : b200seg_make_act_tmap(&p.tm_side, a.res, a.r_ld, a.r_coff, a.Cout, a.B * a.D, a.H, a.W, TW, TH, p.NT / epp, epp, f32);
     if (!ok) return B200SEG_ECUDA;       // conv3d_fwd_tc_supported checked every other condition of the map
   }
   // shared memory carve-up
@@ -677,7 +719,7 @@ int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
   const int gnorm_bytes = a.gx ? a.B * a.Cout * 8 : 0;
   const int side_bytes = p.SS * p.side_stage_bytes;
   const int budget = 227 * 1024 - 1024 - norm_bytes - gnorm_bytes - side_bytes - 512;
-  const int64_t w_total = (int64_t)a.kd * a.kh * a.kw * a.Cin * a.Cout * 2;
+  const int64_t w_total = (int64_t)a.kd * a.kh * a.kw * a.Cin * a.Cout * es;
   int b_region;
   if (w_total <= 112 * 1024 && w_total + 2 * p.a_stage_bytes <= budget) {
     p.w_resident = 1; p.SB = 1;
@@ -710,7 +752,10 @@ int conv3d_fwd_tc(const ConvArgs& a, int dtype, cudaStream_t st) {
   int grid = p.n_tiles < B200SEG_NUM_SMS ? p.n_tiles : B200SEG_NUM_SMS;
   int rc = B200SEG_OK;
   dispatch_n(p.NT, [&](auto nt) {
-    dispatch_ksteps(p.KC / 16, [&](auto ks) { rc = launch_conv_tc<decltype(nt)::value, decltype(ks)::value>(p, grid, smem_bytes, st); });
+    dispatch_ksteps(p.KC / (2 * epp), [&](auto ks) {
+      if (f32) rc = launch_conv_tc<float, decltype(nt)::value, decltype(ks)::value>(p, grid, smem_bytes, st);
+      else rc = launch_conv_tc<__half, decltype(nt)::value, decltype(ks)::value>(p, grid, smem_bytes, st);
+    });
   });
   return rc;
 }

@@ -104,6 +104,27 @@ __device__ __forceinline__ uint4 norm_act8(uint4 raw, const float (&sc)[8], cons
   return raw;
 }
 
+// fp32 -> the nearest TF32 value (round to nearest, ties away from zero), kept in fp32 storage with the low 13 mantissa
+// bits zero: what the library writes as a TF32 operand, so the tensor core's own treatment of those bits never matters
+__device__ __forceinline__ float round_tf32(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return __uint_as_float(r);
+}
+
+// The fp32 form of norm_act8: one 16-byte chunk holds 4 fp32 channels; the result is rounded to TF32.
+template <bool RELU>
+__device__ __forceinline__ uint4 norm_act4(uint4 raw, const float (&sc)[4], const float (&sf)[4], float slope) {
+  float* fv = reinterpret_cast<float*>(&raw);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float f = fmaf(fv[j], sc[j], sf[j]);
+    f = RELU ? fmaxf(f, 0.f) : act_apply_s(f, slope);
+    fv[j] = round_tf32(f);
+  }
+  return raw;
+}
+
 // Calls f(std::integral_constant<int, N>{}) for the run-time GEMM N of a consumer warpgroup (a multiple of 16 up to
 // 128): the one place where an operand width becomes a template argument (of a kernel on the host, of a role on the
 // device).  The caller's lambda is host-only or device-only; the check is disabled so neither side warns about the other.

@@ -10,7 +10,7 @@ so fused tensors (conv1+shortcut outputs, concat buffers) are consumed in place.
 import torch
 
 from . import _lib
-from ._lib import ACT_NONE, ACT_RELU, ALGO_AUTO, ALGO_DIRECT, ALGO_TC, F16, F32, call
+from ._lib import ACT_NONE, ACT_RELU, ALGO_AUTO, ALGO_DIRECT, ALGO_TC, ALGO_TC_TF32, F16, F32, call
 
 IN_EPS = 1e-4  # nn.InstanceNorm3d(eps=1e-4): reference conv_layers.py:40,42
 
@@ -103,10 +103,24 @@ def new_stats(B, C, device):
 
 
 # ----------------------------------------------------------------------------- raw launches
+def tf32_enabled():
+    """True when torch allows TF32 for fp32 matmuls (torch.backends.cuda.matmul.fp32_precision == 'tf32'), read at call
+    time.  The convolutions and Linears here are implicit GEMMs, so they follow torch's matmul precision — not cuDNN's
+    conv flag, which defaults to TF32 — and stay exact fp32 unless the user opts in.  Only `fp32_precision` is read:
+    after the new precision API has been used, the legacy getters raise."""
+    return torch.backends.cuda.matmul.fp32_precision == "tf32"
+
+
 def conv_algo(Cin, Cout, ksize, dtype, B=1):
-    """Algorithm (ALGO_TC / ALGO_DIRECT) the library uses for this conv shape; also names the packed-weight layout."""
-    return _lib.load().b200seg_conv3d_algo(Cin, Cout, ksize[0], ksize[1], ksize[2],
-                                           F16 if dtype == torch.float16 else F32, B)
+    """Algorithm (ALGO_TC / ALGO_TC_TF32 / ALGO_DIRECT) the library uses for this conv shape; also names the
+    packed-weight layout.  fp32 shapes take the TF32 tensor cores only while `tf32_enabled()`."""
+    lib = _lib.load()
+    if dtype != torch.float16 and tf32_enabled():
+        return lib.b200seg_conv3d_algo_tf32(Cin, Cout, ksize[0], ksize[1], ksize[2], B)
+    return lib.b200seg_conv3d_algo(Cin, Cout, ksize[0], ksize[1], ksize[2], F16 if dtype == torch.float16 else F32, B)
+
+
+_LAYOUT_CODE = {ALGO_DIRECT: 0, ALGO_TC: 1, ALGO_TC_TF32: 2}     # the job column of b200seg_pack_weights_multi
 
 
 def pack_weight(w, dtype, transpose_flip=False, out=None, co_off=0, co_total=None, layout=ALGO_DIRECT):
@@ -224,7 +238,9 @@ class PackedWeights:
       * a holder attached to a ``PackRegistry`` (every b200seg model attaches its holders) is refreshed by the
         registry's single multi-tensor launch at the top of ``model.forward`` (≈60 us for 40 M parameters);
       * a free-standing holder (unit tests driving one block) re-packs inside ``get`` with per-weight launches.
-    What IS cached is the allocation and the job description, keyed on (dtype, B, co_pad, data_ptrs, shapes)."""
+    What IS cached is the allocation and the job description, keyed on (dtype, B, co_pad, the two algorithms,
+    data_ptrs, shapes): the algorithms name the image layouts, so toggling TF32 repacks instead of handing one kernel
+    the other's image."""
 
     def __init__(self):
         self._sig = None
@@ -233,25 +249,37 @@ class PackedWeights:
         self._jobs = []           # [(weight, out tensor, transpose_flip, co_off, co_total, layout)]
         self._registry = None
         self._epoch = -1
+        self._algo_key = None     # (dtype, B, co_pad, shapes, TF32 allowed) the cached algorithms were chosen for
+        self._algo_pair = None
 
-    def _signature(self, weights, dtype, B, co_pad):
-        return (dtype, B, co_pad) + tuple((w.data_ptr(), tuple(w.shape)) for w in weights)
+    def _algos(self, weights, dtype, B, co_pad):
+        """(forward, data-gradient) algorithms, asked of the library only when an input of the choice changed"""
+        key = (dtype, B, co_pad, tuple(tuple(w.shape) for w in weights), dtype != torch.float16 and tf32_enabled())
+        if key != self._algo_key:
+            co_total = sum(w.shape[0] for w in weights) + co_pad
+            Cin, ks = weights[0].shape[1], tuple(weights[0].shape[2:])
+            self._algo_key = key
+            self._algo_pair = (conv_algo(Cin, co_total, ks, dtype, B),
+                               conv_algo(co_total, Cin, ks, dtype, B))      # dgrad: channels swap roles
+        return self._algo_pair
+
+    def _signature(self, weights, dtype, B, co_pad, algos):
+        return (dtype, B, co_pad, algos) + tuple((w.data_ptr(), tuple(w.shape)) for w in weights)
 
     def get(self, weights, dtype, B=1, co_pad=0):
         """co_pad extra all-zero output channels are appended (Cout not a multiple of 8/16, e.g. the 27 map codes
         or 14 classes of MedFormer) so the wide-tile kernels and 16-byte stores apply; callers ignore them."""
-        sig = self._signature(weights, dtype, B, co_pad)
+        algos = self._algos(weights, dtype, B, co_pad)
+        sig = self._signature(weights, dtype, B, co_pad, algos)
         reg = self._registry
         if sig == self._sig and reg is not None and self._epoch == reg.epoch:
             return self._fwd, self._bwd           # refreshed by the registry's launch of this forward
         if sig != self._sig:
             co_total = sum(w.shape[0] for w in weights) + co_pad
             Cin = weights[0].shape[1]
-            ks = tuple(weights[0].shape[2:])
             taps = weights[0][0, 0].numel()
             dev = weights[0].device
-            algo_f = conv_algo(Cin, co_total, ks, dtype, B)
-            algo_b = conv_algo(co_total, Cin, ks, dtype, B)      # dgrad: channels swap roles
+            algo_f, algo_b = algos
             alloc = torch.zeros if co_pad else torch.empty
             fwd = alloc(taps * co_total * Cin, dtype=dtype, device=dev)
             bwd = alloc(taps * co_total * Cin, dtype=dtype, device=dev)
@@ -305,7 +333,7 @@ class PackRegistry:
                     taps = w[0, 0].numel()
                     j = len(jobs)
                     jobs.append([w.data_ptr(), out.data_ptr(), w.shape[0], w.shape[1], taps, _dt(out),
-                                 1 if flip else 0, off, co_total, 1 if layout == ALGO_TC else 0])
+                                 1 if flip else 0, off, co_total, _LAYOUT_CODE[layout]])
                     tile_ci = lib.b200seg_pack_tile_ci(taps)
                     if tile_ci and w.shape[0] % 8 == 0 and w.shape[1] % 8 == 0 and off % 8 == 0 and w.shape[1] < 65536:
                         # TILE chunks: 8 output channels x tile_ci input channels x all taps per block (16-byte stores)

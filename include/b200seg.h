@@ -48,9 +48,12 @@ enum {
   B200SEG_ENODEVICE = -4    /* device is not sm_90 (this library has no fallback)            */
 };
 
-/* conv algorithms.  conv3d_fwd takes TC or DIRECT (whatever b200seg_conv3d_algo returned when the
- * weights were packed); wgrad also accepts AUTO since it consumes no packed weights. */
-enum { B200SEG_ALGO_AUTO = 0, B200SEG_ALGO_DIRECT = 1, B200SEG_ALGO_TC = 2 };
+/* conv algorithms.  conv3d_fwd takes TC, TC_TF32 or DIRECT (whatever b200seg_conv3d_algo /
+ * b200seg_conv3d_algo_tf32 returned when the weights were packed); wgrad also accepts AUTO since it
+ * consumes no packed weights.  TC runs fp16 operands; TC_TF32 runs fp32 tensors on the same
+ * tensor-core kernel with TF32 operands (dtype = B200SEG_F32 only) and is never chosen unless the
+ * caller asks for it. */
+enum { B200SEG_ALGO_AUTO = 0, B200SEG_ALGO_DIRECT = 1, B200SEG_ALGO_TC = 2, B200SEG_ALGO_TC_TF32 = 3 };
 
 /* activation applied to the (optionally normalised) conv input in the loader */
 enum { B200SEG_ACT_NONE = 0, B200SEG_ACT_RELU = 1,
@@ -139,7 +142,8 @@ int b200seg_instnorm_bwd_apply(const void* g, int g_ld, int g_coff,
  * transpose_flip!=0 builds the dgrad operand instead:
  *   w_packed[T-1-tap][Cin][Cout] (roles of Cin/Cout swapped, taps mirrored).
  * co_off / co_total place this weight's output channels inside a wider fused
- * weight (conv1+shortcut of a BasicBlock share one GEMM, conv_layers.py:79,84). */
+ * weight (conv1+shortcut of a BasicBlock share one GEMM, conv_layers.py:79,84).
+ * layout is B200SEG_ALGO_DIRECT, _TC (dtype F16) or _TC_TF32 (dtype F32). */
 int b200seg_pack_weight(const float* w, int Cout, int Cin, int taps,
                         void* w_packed, int dtype, int transpose_flip,
                         int co_off, int co_total, int layout, void* stream);
@@ -148,7 +152,8 @@ int b200seg_pack_weight(const float* w, int Cout, int Cin, int taps,
  * model (called once per forward, so an in-place `.data` update of a parameter —
  * the reference's EMA, training/utils.py:99-102 — can never leave a stale image).
  *   jobs_dev  : int64 [njobs][10] = {w ptr, out ptr, Cout, Cin, taps, dtype,
- *               transpose_flip, co_off, co_total, layout==TC}
+ *               transpose_flip, co_off, co_total, layout code}; layout code 0 = DIRECT,
+ *               1 = TC, 2 = TC_TF32
  *   chunks_dev: int64 [nchunks][2] = {job index, code}, one thread block each:
  *               code >= 0: ELEMENT chunk, b200seg_pack_chunk_elems() consecutive elements of w
  *                          starting at `code`;
@@ -164,10 +169,16 @@ int b200seg_pack_weights_multi(const int64_t* jobs_dev, const int64_t* chunks_de
 
 /* Which algorithm (B200SEG_ALGO_TC or _DIRECT) serves a conv of this shape.  The
  * packed-weight layout is per algorithm (`layout` above = this value):
- *   DIRECT: [tap][Cout][Cin];
- *   TC    : the shared-memory image the tensor-core kernel streams with bulk TMA,
- *           [ntile][tap][kchunk][KC/8][NT][8]  (NT / KC: csrc/conv_args.h). */
+ *   DIRECT : [tap][Cout][Cin];
+ *   TC     : the shared-memory image the tensor-core kernel streams with bulk TMA,
+ *            [ntile][tap][kchunk][KC/8][NT][8] fp16  (NT / KC: csrc/conv_args.h);
+ *   TC_TF32: the same image in 16-byte planes of 4 fp32 channels, rounded to TF32,
+ *            [ntile][tap][kchunk][KC/4][NT][4]  (KC: tc_pick_kc_tf32).
+ * fp32 convolutions are always DIRECT here: TF32 is an opt-in (b200seg_conv3d_algo_tf32). */
 int b200seg_conv3d_algo(int Cin, int Cout, int kd, int kh, int kw, int dtype, int B);
+/* TC_TF32 when an fp32 conv of this shape can run on TF32 tensor cores (same kernel-size and
+ * batch limits as the fp16 rule; Cin a multiple of 8, Cout of 16), else DIRECT. */
+int b200seg_conv3d_algo_tf32(int Cin, int Cout, int kd, int kh, int kw, int B);
 
 /* y[.., y_coff:y_coff+Cout] = conv(act(IN(x))) (+bias) (+residual); optionally
  * accumulates InstanceNorm sums of the STORED y into y_stats.
