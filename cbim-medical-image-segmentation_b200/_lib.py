@@ -98,10 +98,14 @@ _PROTOS = {
     "b200seg_biattn_fwd": [P, I, I, P, I, I, P, I, P, I, I, P, I, I, P, I, I, P, P, I, L, I, I, I, F, I, P],
     "b200seg_biattn_bwd": [P, I, I, P, I, I, P, I, P, I, I, P, I, I, P, P, I, I, P, I, I, P, I, I, P, I, I,
                            P, I, P, I, I, P, I, L, I, I, I, F, I, P],
+    "b200seg_biattn_wide_workspace": [I, L, I, I, I],
+    "b200seg_biattn_wide_fwd": [P, I, I, P, I, I, P, I, P, I, I, P, I, I, P, I, I, P, P, I, L, I, I, I, F, I, P],
+    "b200seg_biattn_wide_bwd": [P, I, I, P, I, I, P, I, P, I, I, P, I, I, P, P, I, I, P, I, I, P, I, I, P, I, I,
+                                P, I, P, I, I, P, I, L, I, I, I, F, I, P],
 }
 _RESTYPES = {"b200seg_strerror": c_char_p, "b200seg_last_cuda_error": c_char_p,
              "b200seg_conv3d_wgrad_workspace": ctypes.c_size_t, "b200seg_conv3d_wgrad_pc_workspace": ctypes.c_size_t, "b200seg_biattn_workspace": ctypes.c_size_t,
-             "b200seg_mapgen_workspace": ctypes.c_size_t,
+             "b200seg_mapgen_workspace": ctypes.c_size_t, "b200seg_biattn_wide_workspace": ctypes.c_size_t,
              "b200seg_channel_scale_bwd_workspace": ctypes.c_size_t, "b200seg_window_attn_workspace": ctypes.c_size_t,
              "b200seg_surface_distance_workspace": ctypes.c_size_t, "b200seg_aug2d_workspace": ctypes.c_size_t}
 
@@ -143,7 +147,7 @@ def check(rc, what):
 # kernels launched per entry point (dice fwd = reduce + finalize; its memset is not ours)
 _KERNELS = {"b200seg_dice_ce_fwd": 2, "b200seg_biattn_fwd": 2, "b200seg_window_attn_bwd": 2, "b200seg_attention_bwd": 3, "b200seg_adamw_ema_step": 2, "b200seg_biattn_bwd": 2,
             "b200seg_mapgen_fwd": 2, "b200seg_channel_scale_bwd_reduce": 2, "b200seg_attn_gate_fwd": 2, "b200seg_attn_gate_bwd": 2,
-            "b200seg_aug2d_train": 3}
+            "b200seg_aug2d_train": 3, "b200seg_biattn_wide_fwd": 2, "b200seg_biattn_wide_bwd": 2}
 launch_count = 0
 
 

@@ -451,3 +451,432 @@ extern "C" int b200seg_biattn_bwd(const void* fq, int fq_ld, int fq_coff, const 
   B200_CHECK_LAUNCH("biattn_bwd");
   return B200SEG_OK;
 }
+
+// ------------------------------------------------------------------------------------------------------------------
+// Wide B-MHA: dim_head 32 / 64 / 80 over up to 80 map tokens (ACDC's 2x6x6 = 72 maps at dim_head 32, 64 and 80),
+// for every shape the entry points above refuse.  The one-voxel-per-thread layout above keeps S[M], v[DH] and dv[DH]
+// in registers, which spills at 80 x 80.  Here a block owns WT = 64 voxels and every operand lives in shared memory:
+// the voxel tiles [WT][DH], the map operands [MP][DH] (zero-padded to MP = 80 tokens) and the score-shaped tiles
+// [WT][MP].  Each contraction is a small register-tiled product between two of them (20 or 25 accumulators per thread),
+// so no thread holds a dim_head- or token-long array.  The column softmax and its merge are those of the kernels above.
+namespace {
+
+constexpr int WT = 64;             // voxels per block
+constexpr int WTHREADS = 256;
+constexpr int MP = 80;             // map-token rows of the shared operands
+constexpr int SLD = MP + 1;        // row stride of the score-shaped tiles (odd: conflict-free per-voxel rows)
+
+template <int DH> struct WideCfg {
+  static constexpr int LD = DH + 4;                  // row stride of the [*][DH] tiles: 16-byte rows
+  static constexpr int NW = DH / 4;                  // channels per thread in the voxel-major products
+  static constexpr int CW = DH / 16;                 // channels per thread in the token-major products
+};
+
+// out[i][j] = alpha * <A_i, B_j> for the WT voxels x MP tokens; thread = (voxel i, a warp-uniform group of 20 tokens)
+template <int DH>
+__device__ __forceinline__ void wide_nt(const float* A, const float* Bm, float* out, float alpha) {
+  constexpr int LD = WideCfg<DH>::LD;
+  const int i = threadIdx.x & (WT - 1), j0 = (threadIdx.x >> 6) * 20;
+  float acc[20];
+#pragma unroll
+  for (int t = 0; t < 20; ++t) acc[t] = 0.f;
+#pragma unroll 2
+  for (int d0 = 0; d0 < DH; d0 += 4) {
+    const float4 a = *reinterpret_cast<const float4*>(A + i * LD + d0);
+#pragma unroll
+    for (int t = 0; t < 20; ++t) acc[t] = dot4(a.x, a.y, a.z, a.w, *reinterpret_cast<const float4*>(Bm + (j0 + t) * LD + d0), acc[t]);
+  }
+#pragma unroll
+  for (int t = 0; t < 20; ++t) out[i * SLD + j0 + t] = acc[t] * alpha;
+}
+
+// acc[c] = sum_{j<M} P[i][j] * Bm[j][d0 + c] for the thread's voxel i = tid % WT and channels d0 = (tid / WT) * NW ..
+template <int DH>
+__device__ __forceinline__ void wide_nn(const float* P, const float* Bm, int M, float (&acc)[WideCfg<DH>::NW]) {
+  constexpr int LD = WideCfg<DH>::LD, NW = WideCfg<DH>::NW;
+  const int i = threadIdx.x & (WT - 1), d0 = (threadIdx.x >> 6) * NW;
+#pragma unroll
+  for (int c = 0; c < NW; ++c) acc[c] = 0.f;
+  for (int j = 0; j < M; ++j) {
+    const float p = P[i * SLD + j];
+#pragma unroll
+    for (int c = 0; c < NW; c += 4) {
+      const float4 w = *reinterpret_cast<const float4*>(Bm + j * LD + d0 + c);
+      acc[c] = fmaf(p, w.x, acc[c]); acc[c + 1] = fmaf(p, w.y, acc[c + 1]);
+      acc[c + 2] = fmaf(p, w.z, acc[c + 2]); acc[c + 3] = fmaf(p, w.w, acc[c + 3]);
+    }
+  }
+}
+
+// acc[t][c] = sum_{i<WT} P[i][j0 + t] * X[i][d0 + c]; thread = (5 tokens j0 = (tid / 16) * 5, CW channels d0 = (tid % 16) * CW)
+template <int DH>
+__device__ __forceinline__ void wide_tn(const float* P, const float* X, float (&acc)[5][WideCfg<DH>::CW]) {
+  constexpr int LD = WideCfg<DH>::LD, CW = WideCfg<DH>::CW;
+  const int j0 = (threadIdx.x >> 4) * 5, d0 = (threadIdx.x & 15) * CW;
+#pragma unroll
+  for (int t = 0; t < 5; ++t)
+#pragma unroll
+    for (int c = 0; c < CW; ++c) acc[t][c] = 0.f;
+#pragma unroll 2
+  for (int i = 0; i < WT; ++i) {
+    float p[5], x[CW];
+#pragma unroll
+    for (int t = 0; t < 5; ++t) p[t] = P[i * SLD + j0 + t];
+#pragma unroll
+    for (int c = 0; c < CW; ++c) x[c] = X[i * LD + d0 + c];
+#pragma unroll
+    for (int t = 0; t < 5; ++t)
+#pragma unroll
+      for (int c = 0; c < CW; ++c) acc[t][c] = fmaf(p[t], x[c], acc[t][c]);
+  }
+}
+
+// [rows][DH] operand rows r < nrows of channel d*heads + h, scaled; rows >= nrows (and the stride padding) zero
+template <typename T, int DH>
+__device__ __forceinline__ void wide_stage(float* dst, int rows, const T* src, int64_t row0, int64_t ld, int nrows,
+                                           int heads, int h, float alpha) {
+  constexpr int LD = WideCfg<DH>::LD;
+  for (int o = threadIdx.x; o < rows * LD; o += WTHREADS) {
+    const int r = o / LD, d = o % LD;
+    dst[o] = (r < nrows && d < DH) ? Elem<T>::ld(src + (row0 + r) * ld + d * heads + h) * alpha : 0.f;
+  }
+}
+
+template <typename T, int DH>
+__global__ void __launch_bounds__(WTHREADS)
+biattn_wide_fwd_kernel(BiArgs a) {
+  using C = WideCfg<DH>;
+  extern __shared__ float sm[];
+  float* s_qm = sm;                        // [MP][LD] pre-scaled map queries
+  float* s_vm = s_qm + MP * C::LD;         // [MP][LD]
+  float* s_qf = s_vm + MP * C::LD;         // [WT][LD]
+  float* s_vf = s_qf + WT * C::LD;         // [WT][LD]
+  float* s_s = s_vf + WT * C::LD;          // [WT][SLD] scores, then the row softmax
+  float* s_e = s_s + WT * SLD;             // [WT][SLD] exp(S - block column max)
+  float* s_cmax = s_e + WT * SLD;          // [MP]
+  float* s_row = s_cmax + MP;              // [WT][2] row max, 1 / row sum
+  const int h = blockIdx.y, b = blockIdx.z, M = a.M, heads = a.heads, tid = threadIdx.x;
+  const int64_t i0 = (int64_t)blockIdx.x * WT;
+  const int nv = (int)min((int64_t)WT, a.N - i0);
+  wide_stage<T, DH>(s_qm, MP, (const T*)a.mq + a.mq_coff, (int64_t)b * M, a.m_ld, M, heads, h, a.scale);
+  wide_stage<T, DH>(s_vm, MP, (const T*)a.mv + a.mv_coff, (int64_t)b * M, a.m_ld, M, heads, h, 1.f);
+  wide_stage<T, DH>(s_qf, WT, (const T*)a.fq + a.fq_coff, (int64_t)b * a.N + i0, a.fq_ld, nv, heads, h, 1.f);
+  wide_stage<T, DH>(s_vf, WT, (const T*)a.fv + a.fv_coff, (int64_t)b * a.N + i0, a.fv_ld, nv, heads, h, 1.f);
+  __syncthreads();
+  wide_nt<DH>(s_qf, s_qm, s_s, 1.f);
+  __syncthreads();
+  if (tid < M) {                                            // column max over the block's voxels
+    float m = -INFINITY;
+    for (int i = 0; i < nv; ++i) m = fmaxf(m, s_s[i * SLD + tid]);
+    s_cmax[tid] = m;
+  } else if (tid >= 128 && tid < 128 + nv) {                // row softmax statistics
+    const int i = tid - 128;
+    float m = -INFINITY, sum = 0.f;
+    for (int j = 0; j < M; ++j) m = fmaxf(m, s_s[i * SLD + j]);
+    for (int j = 0; j < M; ++j) sum += __expf(s_s[i * SLD + j] - m);
+    s_row[2 * i] = m; s_row[2 * i + 1] = 1.f / sum;
+  }
+  __syncthreads();
+  for (int o = tid; o < WT * MP; o += WTHREADS) {
+    const int i = o / MP, j = o % MP;
+    const bool ok = i < nv && j < M;
+    const float s = s_s[i * SLD + j];
+    s_e[i * SLD + j] = ok ? __expf(s - s_cmax[j]) : 0.f;
+    s_s[i * SLD + j] = ok ? __expf(s - s_row[2 * i]) * s_row[2 * i + 1] : 0.f;
+  }
+  __syncthreads();
+  {
+    float acc[C::NW];
+    wide_nn<DH>(s_s, s_vm, M, acc);
+    const int i = tid & (WT - 1), d0 = (tid >> 6) * C::NW;
+    if (i < nv) {
+      T* op = (T*)a.fo + ((int64_t)b * a.N + i0 + i) * a.fo_ld + a.fo_coff + h;
+#pragma unroll
+      for (int c = 0; c < C::NW; ++c) Elem<T>::st(op + (d0 + c) * heads, acc[c]);
+    }
+  }
+  {
+    float acc[5][C::CW];
+    wide_tn<DH>(s_e, s_vf, acc);
+    const int nblk = gridDim.x, j0 = (tid >> 4) * 5, d0 = (tid & 15) * C::CW;
+    float* pb = a.partial + ((((int64_t)b * heads + h) * nblk + blockIdx.x) * M) * (2 + DH);
+#pragma unroll
+    for (int t = 0; t < 5; ++t)
+      if (j0 + t < M)
+#pragma unroll
+        for (int c = 0; c < C::CW; ++c) pb[(j0 + t) * (2 + DH) + 2 + d0 + c] = acc[t][c];
+    if (tid < M) {
+      float esum = 0.f;
+      for (int i = 0; i < nv; ++i) esum += s_e[i * SLD + tid];
+      pb[tid * (2 + DH)] = s_cmax[tid]; pb[tid * (2 + DH) + 1] = esum;
+    }
+  }
+}
+
+// the forward merge of biattn_fwd_merge_kernel for DH channels: 4 partitions of the block axis x 32 lanes, each lane
+// owning channels lane, lane + 32, lane + 64 (< DH)
+template <typename T, int DH>
+__global__ void biattn_wide_fwd_merge_kernel(BiArgs a, int nblk) {
+  constexpr int NC = (DH + 31) / 32;
+  const int j = blockIdx.x, h = blockIdx.y, b = blockIdx.z, M = a.M, heads = a.heads;
+  const int lane = threadIdx.x & 31, part = threadIdx.x >> 5;
+  const float* pb = a.partial + ((((int64_t)b * heads + h) * nblk) * M + j) * (2 + DH);
+  float m = -INFINITY, sum = 0.f, acc[NC];
+#pragma unroll
+  for (int u = 0; u < NC; ++u) acc[u] = 0.f;
+  for (int k = part; k < nblk; k += 4) {
+    const float* q = pb + (int64_t)k * M * (2 + DH);
+    const float mk = q[0];
+    if (mk > m) {
+      const float sc = __expf(m - mk);
+      sum *= sc;
+#pragma unroll
+      for (int u = 0; u < NC; ++u) acc[u] *= sc;
+      m = mk;
+    }
+    const float e = __expf(mk - m);
+    sum = fmaf(q[1], e, sum);
+#pragma unroll
+    for (int u = 0; u < NC; ++u) if (lane + 32 * u < DH) acc[u] = fmaf(q[2 + lane + 32 * u], e, acc[u]);
+  }
+  __shared__ float s_m[4], s_s[4], s_a[4][NC * 32];
+  if (lane == 0) { s_m[part] = m; s_s[part] = sum; }
+#pragma unroll
+  for (int u = 0; u < NC; ++u) s_a[part][lane + 32 * u] = acc[u];
+  __syncthreads();
+  if (part == 0) {
+    const float gm = fmaxf(fmaxf(s_m[0], s_m[1]), fmaxf(s_m[2], s_m[3]));
+    float gs = 0.f, ga[NC];
+#pragma unroll
+    for (int u = 0; u < NC; ++u) ga[u] = 0.f;
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+      const float e = __expf(s_m[p] - gm);
+      gs = fmaf(s_s[p], e, gs);
+#pragma unroll
+      for (int u = 0; u < NC; ++u) ga[u] = fmaf(s_a[p][lane + 32 * u], e, ga[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < NC; ++u) {
+      const int d = lane + 32 * u;
+      if (d < DH) Elem<T>::st((T*)a.mo + ((int64_t)b * M + j) * a.mo_ld + a.mo_coff + d * heads + h, ga[u] / gs);
+    }
+    if (lane == 0) { float* cs = a.colstat + (((int64_t)b * heads + h) * M + j) * 2; cs[0] = gm; cs[1] = gs; }
+  }
+}
+
+template <typename T, int DH>
+__global__ void __launch_bounds__(WTHREADS)
+biattn_wide_bwd_kernel(BiArgs a) {
+  using C = WideCfg<DH>;
+  extern __shared__ float sm[];
+  float* s_qm = sm;                        // [MP][LD] (unscaled)
+  float* s_vm = s_qm + MP * C::LD;
+  float* s_dmo = s_vm + MP * C::LD;
+  float* s_qf = s_dmo + MP * C::LD;        // [WT][LD]
+  float* s_vf = s_qf + WT * C::LD;
+  float* s_do = s_vf + WT * C::LD;
+  float* s_p1 = s_do + WT * C::LD;         // [WT][SLD] scores, then the row softmax p1
+  float* s_ds = s_p1 + WT * SLD;           // [WT][SLD] dA1, then dS
+  float* s_p2 = s_ds + WT * SLD;           // [WT][SLD] dA2, then the column softmax p2
+  float* s_col = s_p2 + WT * SLD;          // [MP][3] gmax, 1 / gsum, c_j
+  float* s_row = s_col + 3 * MP;           // [WT][3] row max, 1 / row sum, t1
+  const int h = blockIdx.y, b = blockIdx.z, M = a.M, heads = a.heads, tid = threadIdx.x;
+  const int64_t i0 = (int64_t)blockIdx.x * WT, row0 = (int64_t)b * a.N + i0;
+  const int nv = (int)min((int64_t)WT, a.N - i0);
+  wide_stage<T, DH>(s_qm, MP, (const T*)a.mq + a.mq_coff, (int64_t)b * M, a.m_ld, M, heads, h, 1.f);
+  wide_stage<T, DH>(s_vm, MP, (const T*)a.mv + a.mv_coff, (int64_t)b * M, a.m_ld, M, heads, h, 1.f);
+  wide_stage<T, DH>(s_dmo, MP, (const T*)a.dmo + a.dmo_coff, (int64_t)b * M, a.dmo_ld, M, heads, h, 1.f);
+  wide_stage<T, DH>(s_qf, WT, (const T*)a.fq + a.fq_coff, row0, a.fq_ld, nv, heads, h, 1.f);
+  wide_stage<T, DH>(s_vf, WT, (const T*)a.fv + a.fv_coff, row0, a.fv_ld, nv, heads, h, 1.f);
+  wide_stage<T, DH>(s_do, WT, (const T*)a.dfo + a.dfo_coff, row0, a.dfo_ld, nv, heads, h, 1.f);
+  __syncthreads();
+  if (tid < M) {                           // c_j = <dmap_out_j, map_out_j>
+    const float* cs = a.colstat + (((int64_t)b * heads + h) * M + tid) * 2;
+    const T* mo = (const T*)a.mo + ((int64_t)b * M + tid) * a.mo_ld + a.mo_coff + h;
+    float c = 0.f;
+    for (int d = 0; d < DH; ++d) c = fmaf(s_dmo[tid * C::LD + d], Elem<T>::ld(mo + d * heads), c);
+    s_col[3 * tid] = cs[0]; s_col[3 * tid + 1] = 1.f / cs[1]; s_col[3 * tid + 2] = c;
+  }
+  wide_nt<DH>(s_qf, s_qm, s_p1, a.scale);  // S
+  wide_nt<DH>(s_do, s_vm, s_ds, 1.f);      // dA1_ij = <dO_i, Vm_j>
+  wide_nt<DH>(s_vf, s_dmo, s_p2, 1.f);     // dA2_ij = <Vf_i, dmo_j>
+  __syncthreads();
+  if (tid < nv) {
+    float m = -INFINITY, sum = 0.f, t1 = 0.f;
+    for (int j = 0; j < M; ++j) m = fmaxf(m, s_p1[tid * SLD + j]);
+    for (int j = 0; j < M; ++j) {
+      const float e = __expf(s_p1[tid * SLD + j] - m);
+      sum += e; t1 = fmaf(e, s_ds[tid * SLD + j], t1);
+    }
+    s_row[3 * tid] = m; s_row[3 * tid + 1] = 1.f / sum; s_row[3 * tid + 2] = t1 / sum;
+  }
+  __syncthreads();
+  for (int o = tid; o < WT * MP; o += WTHREADS) {
+    const int i = o / MP, j = o % MP;
+    float p1 = 0.f, p2 = 0.f, ds = 0.f;
+    if (i < nv && j < M) {
+      const float s = s_p1[i * SLD + j];
+      p1 = __expf(s - s_row[3 * i]) * s_row[3 * i + 1];
+      p2 = __expf(s - s_col[3 * j]) * s_col[3 * j + 1];
+      ds = p1 * (s_ds[i * SLD + j] - s_row[3 * i + 2]) + p2 * (s_p2[i * SLD + j] - s_col[3 * j + 2]);
+    }
+    s_p1[i * SLD + j] = p1; s_p2[i * SLD + j] = p2; s_ds[i * SLD + j] = ds;
+  }
+  __syncthreads();
+  {
+    const int i = tid & (WT - 1), d0 = (tid >> 6) * C::NW;
+    float acc[C::NW];
+    wide_nn<DH>(s_ds, s_qm, M, acc);       // dQf = scale * dS Qm
+    if (i < nv) {
+      T* p = (T*)a.dfq + (row0 + i) * a.dfq_ld + a.dfq_coff + h;
+#pragma unroll
+      for (int c = 0; c < C::NW; ++c) Elem<T>::st(p + (d0 + c) * heads, acc[c] * a.scale);
+    }
+    wide_nn<DH>(s_p2, s_dmo, M, acc);      // dVf = p2 dmo
+    if (i < nv) {
+      T* p = (T*)a.dfv + (row0 + i) * a.dfv_ld + a.dfv_coff + h;
+#pragma unroll
+      for (int c = 0; c < C::NW; ++c) Elem<T>::st(p + (d0 + c) * heads, acc[c]);
+    }
+  }
+  {
+    const int nblk = gridDim.x, j0 = (tid >> 4) * 5, d0 = (tid & 15) * C::CW;
+    float* pb = a.partial + ((((int64_t)b * heads + h) * nblk + blockIdx.x) * M) * (2 * DH);
+    float acc[5][C::CW];
+    wide_tn<DH>(s_ds, s_qf, acc);          // dQm partial = scale * dS^T Qf
+#pragma unroll
+    for (int t = 0; t < 5; ++t)
+      if (j0 + t < M)
+#pragma unroll
+        for (int c = 0; c < C::CW; ++c) pb[(j0 + t) * 2 * DH + d0 + c] = acc[t][c] * a.scale;
+    wide_tn<DH>(s_p1, s_do, acc);          // dVm partial = p1^T dO
+#pragma unroll
+    for (int t = 0; t < 5; ++t)
+      if (j0 + t < M)
+#pragma unroll
+        for (int c = 0; c < C::CW; ++c) pb[(j0 + t) * 2 * DH + DH + d0 + c] = acc[t][c];
+  }
+}
+
+// sum of the per-block map-gradient partials in block order: 4 partitions x 64 lanes, lane owning values
+// lane, lane + 64, lane + 128 (< 2 * DH) of [dq | dv]
+template <typename T, int DH>
+__global__ void biattn_wide_bwd_merge_kernel(BiArgs a, int nblk) {
+  constexpr int NC = (2 * DH + 63) / 64;
+  const int j = blockIdx.x, h = blockIdx.y, b = blockIdx.z, M = a.M, heads = a.heads;
+  const int lane = threadIdx.x & 63, part = threadIdx.x >> 6;
+  const float* pb = a.partial + ((((int64_t)b * heads + h) * nblk) * M + j) * (2 * DH);
+  float acc[NC];
+#pragma unroll
+  for (int u = 0; u < NC; ++u) acc[u] = 0.f;
+  for (int k = part; k < nblk; k += 4)
+#pragma unroll
+    for (int u = 0; u < NC; ++u) if (lane + 64 * u < 2 * DH) acc[u] += pb[(int64_t)k * M * (2 * DH) + lane + 64 * u];
+  __shared__ float s_a[4][NC * 64];
+#pragma unroll
+  for (int u = 0; u < NC; ++u) s_a[part][lane + 64 * u] = acc[u];
+  __syncthreads();
+  if (part == 0) {
+#pragma unroll
+    for (int u = 0; u < NC; ++u) {
+      const int c = lane + 64 * u;
+      if (c >= 2 * DH) continue;
+      const float v = s_a[0][c] + s_a[1][c] + s_a[2][c] + s_a[3][c];
+      const int d = c < DH ? c : c - DH;
+      const int64_t off = ((int64_t)b * M + j) * a.dm_ld + d * heads + h;
+      if (c < DH) Elem<T>::st((T*)a.dmq + off + a.dmq_coff, v);
+      else Elem<T>::st((T*)a.dmv + off + a.dmv_coff, v);
+    }
+  }
+}
+
+template <int DH> constexpr size_t wide_fwd_smem() { return sizeof(float) * (2 * MP * WideCfg<DH>::LD + 2 * WT * WideCfg<DH>::LD + 2 * WT * SLD + MP + 2 * WT); }
+template <int DH> constexpr size_t wide_bwd_smem() { return sizeof(float) * (3 * MP * WideCfg<DH>::LD + 3 * WT * WideCfg<DH>::LD + 3 * WT * SLD + 3 * MP + 3 * WT); }
+
+}  // namespace
+
+// the shapes b200seg_biattn_fwd / _bwd do not take: dim_head 32 with 65..80 tokens, dim_head 64 / 80 with 1..80
+static int check_wide_args(int B, int64_t N, int M, int heads, int dim_head, int dtype) {
+  if (B <= 0 || N <= 0 || M <= 0 || heads <= 0) return B200SEG_EINVAL;
+  if (dtype != B200SEG_F16 && dtype != B200SEG_F32) return B200SEG_EINVAL;
+  if (dim_head != 32 && dim_head != 64 && dim_head != 80) return B200SEG_EUNSUPPORTED;
+  if (M > MP || (dim_head == DH && M <= MAXM_CAP)) return B200SEG_EUNSUPPORTED;
+  if ((N + WT - 1) / WT > 2147483647LL || heads > 65535 || B > 65535) return B200SEG_EUNSUPPORTED;
+  return B200SEG_OK;
+}
+
+extern "C" size_t b200seg_biattn_wide_workspace(int B, int64_t N, int M, int heads, int dim_head) {
+  const int64_t nblk = (N + WT - 1) / WT;
+  return (size_t)B * heads * nblk * M * (2 * dim_head) * sizeof(float);
+}
+
+extern "C" int b200seg_biattn_wide_fwd(const void* fq, int fq_ld, int fq_coff, const void* fv, int fv_ld, int fv_coff,
+                                       const void* mq, int mq_coff, const void* mv, int mv_coff, int m_ld,
+                                       void* fo, int fo_ld, int fo_coff, void* mo, int mo_ld, int mo_coff,
+                                       float* colstat, float* workspace, int B, int64_t N, int M, int heads,
+                                       int dim_head, float scale, int dtype, void* stream) {
+  int rc = check_wide_args(B, N, M, heads, dim_head, dtype);
+  if (rc) return rc;
+  if (!fq || !fv || !mq || !mv || !fo || !mo || !colstat || !workspace) return B200SEG_EINVAL;
+  BiArgs a; memset(&a, 0, sizeof(a));
+  a.fq = fq; a.fq_ld = fq_ld; a.fq_coff = fq_coff; a.fv = fv; a.fv_ld = fv_ld; a.fv_coff = fv_coff;
+  a.mq = mq; a.mv = mv; a.m_ld = m_ld; a.mq_coff = mq_coff; a.mv_coff = mv_coff;
+  a.fo = fo; a.fo_ld = fo_ld; a.fo_coff = fo_coff; a.mo = mo; a.mo_ld = mo_ld; a.mo_coff = mo_coff;
+  a.colstat = colstat; a.partial = workspace; a.B = B; a.N = N; a.M = M; a.heads = heads; a.scale = scale;
+  cudaStream_t st = as_stream(stream);
+  const int nblk = (int)((N + WT - 1) / WT);
+  dim3 grid(nblk, heads, B);
+#define B200_WIDE_FWD(TT, D)                                                                                   \
+  do {                                                                                                         \
+    constexpr size_t sm = wide_fwd_smem<D>();                                                                  \
+    B200_CUDA(cudaFuncSetAttribute(biattn_wide_fwd_kernel<TT, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); \
+    biattn_wide_fwd_kernel<TT, D><<<grid, WTHREADS, sm, st>>>(a);                                              \
+    biattn_wide_fwd_merge_kernel<TT, D><<<dim3(M, heads, B), 128, 0, st>>>(a, nblk);                           \
+  } while (0)
+#define B200_WIDE_FWD_T(TT) \
+  do { if (dim_head == 32) B200_WIDE_FWD(TT, 32); else if (dim_head == 64) B200_WIDE_FWD(TT, 64); else B200_WIDE_FWD(TT, 80); } while (0)
+  if (dtype == B200SEG_F16) B200_WIDE_FWD_T(__half); else B200_WIDE_FWD_T(float);
+#undef B200_WIDE_FWD_T
+#undef B200_WIDE_FWD
+  B200_CHECK_LAUNCH("biattn_wide_fwd");
+  return B200SEG_OK;
+}
+
+extern "C" int b200seg_biattn_wide_bwd(const void* fq, int fq_ld, int fq_coff, const void* fv, int fv_ld, int fv_coff,
+                                       const void* mq, int mq_coff, const void* mv, int mv_coff, int m_ld,
+                                       const void* mo, int mo_ld, int mo_coff, const float* colstat,
+                                       const void* dfo, int dfo_ld, int dfo_coff, const void* dmo, int dmo_ld, int dmo_coff,
+                                       void* dfq, int dfq_ld, int dfq_coff, void* dfv, int dfv_ld, int dfv_coff,
+                                       void* dmq, int dmq_coff, void* dmv, int dmv_coff, int dm_ld,
+                                       float* workspace, int B, int64_t N, int M, int heads, int dim_head, float scale,
+                                       int dtype, void* stream) {
+  int rc = check_wide_args(B, N, M, heads, dim_head, dtype);
+  if (rc) return rc;
+  if (!fq || !fv || !mq || !mv || !mo || !colstat || !dfo || !dmo || !dfq || !dfv || !dmq || !dmv || !workspace) return B200SEG_EINVAL;
+  BiArgs a; memset(&a, 0, sizeof(a));
+  a.fq = fq; a.fq_ld = fq_ld; a.fq_coff = fq_coff; a.fv = fv; a.fv_ld = fv_ld; a.fv_coff = fv_coff;
+  a.mq = mq; a.mv = mv; a.m_ld = m_ld; a.mq_coff = mq_coff; a.mv_coff = mv_coff;
+  a.mo = const_cast<void*>(mo); a.mo_ld = mo_ld; a.mo_coff = mo_coff; a.colstat = const_cast<float*>(colstat);
+  a.dfo = dfo; a.dfo_ld = dfo_ld; a.dfo_coff = dfo_coff; a.dmo = dmo; a.dmo_ld = dmo_ld; a.dmo_coff = dmo_coff;
+  a.dfq = dfq; a.dfq_ld = dfq_ld; a.dfq_coff = dfq_coff; a.dfv = dfv; a.dfv_ld = dfv_ld; a.dfv_coff = dfv_coff;
+  a.dmq = dmq; a.dmv = dmv; a.dm_ld = dm_ld; a.dmq_coff = dmq_coff; a.dmv_coff = dmv_coff;
+  a.partial = workspace; a.B = B; a.N = N; a.M = M; a.heads = heads; a.scale = scale;
+  cudaStream_t st = as_stream(stream);
+  const int nblk = (int)((N + WT - 1) / WT);
+  dim3 grid(nblk, heads, B);
+#define B200_WIDE_BWD(TT, D)                                                                                   \
+  do {                                                                                                         \
+    constexpr size_t sm = wide_bwd_smem<D>();                                                                  \
+    B200_CUDA(cudaFuncSetAttribute(biattn_wide_bwd_kernel<TT, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); \
+    biattn_wide_bwd_kernel<TT, D><<<grid, WTHREADS, sm, st>>>(a);                                              \
+    biattn_wide_bwd_merge_kernel<TT, D><<<dim3(M, heads, B), 256, 0, st>>>(a, nblk);                           \
+  } while (0)
+#define B200_WIDE_BWD_T(TT) \
+  do { if (dim_head == 32) B200_WIDE_BWD(TT, 32); else if (dim_head == 64) B200_WIDE_BWD(TT, 64); else B200_WIDE_BWD(TT, 80); } while (0)
+  if (dtype == B200SEG_F16) B200_WIDE_BWD_T(__half); else B200_WIDE_BWD_T(float);
+#undef B200_WIDE_BWD_T
+#undef B200_WIDE_BWD
+  B200_CHECK_LAUNCH("biattn_wide_bwd");
+  return B200SEG_OK;
+}

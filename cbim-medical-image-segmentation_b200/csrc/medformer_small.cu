@@ -5,7 +5,7 @@
 //   channel_scale_*     x * gate                                   conv_layers.py:174
 //   layernorm_fwd/bwd   nn.LayerNorm in PreNorm                    trans_layers.py:36-41
 //   gelu_fwd/bwd        nn.GELU in Mlp                             trans_layers.py:22,28
-//   mhsa_fwd/bwd        Attention over the 81 map tokens           trans_layers.py:45-100
+//   mhsa_fwd/bwd        Attention over the fused map tokens        trans_layers.py:45-100
 // All tensors channels-last; activations in T (fp16/fp32), parameters and statistics fp32/fp64.
 #include "common.cuh"
 
@@ -40,7 +40,7 @@ __global__ void s2d_kernel(const T* __restrict__ x, T* __restrict__ y, int B, in
 }
 
 // ------------------------------------------------------------------ semantic map generation
-constexpr int MG_T = 128, MG_KCAP = 64, MG_CC = 48;   // kernels are built for 32 and 64 map codes
+constexpr int MG_T = 128, MG_KCAP = 80, MG_CC = 48;   // kernels are built for 32, 64 and 80 map codes (80: ACDC's 72)
 
 struct MgArgs {
   const void* f; int f_ld, f_coff; const void* wl; int w_ld, w_coff;   // features [B][N][*], logits [B][N][*]
@@ -60,12 +60,19 @@ __global__ void __launch_bounds__(MG_T) mapgen_fwd_kernel(MgArgs a) {
   const int64_t i = (int64_t)blockIdx.x * MG_T + tid;
   const bool valid = i < a.N;
   const T* wrow = (const T*)a.wl + ((int64_t)b * a.N + i) * a.w_ld + a.w_coff;
-  float lg[MG_K];
+  // the 64- and 32-code builds keep the row's logits in registers; the 80-code build stages them in its own row of
+  // s_e instead (80 live logits next to the shuffles spill)
+  float lg[MG_K > 64 ? 1 : MG_K];
+  if constexpr (MG_K > 64) {
+    for (int k = 0; k < MG_K; ++k) s_e[tid][k] = (valid && k < K) ? Elem<T>::ld(wrow + k) : -INFINITY;
+  } else {
 #pragma unroll
-  for (int k = 0; k < MG_K; ++k) lg[k] = (valid && k < K) ? Elem<T>::ld(wrow + k) : -INFINITY;
+    for (int k = 0; k < MG_K; ++k) lg[k] = (valid && k < K) ? Elem<T>::ld(wrow + k) : -INFINITY;
+  }
 #pragma unroll
   for (int k = 0; k < MG_K; ++k) {
-    float m = lg[k];
+    float m;
+    if constexpr (MG_K > 64) m = s_e[tid][k]; else m = lg[k];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if (lane == 0) s_max[wid][k] = m;
@@ -73,8 +80,12 @@ __global__ void __launch_bounds__(MG_T) mapgen_fwd_kernel(MgArgs a) {
   __syncthreads();
   if (tid < MG_K) s_max[4][tid] = fmaxf(fmaxf(s_max[0][tid], s_max[1][tid]), fmaxf(s_max[2][tid], s_max[3][tid]));
   __syncthreads();
+  if constexpr (MG_K > 64) {
+    for (int k = 0; k < MG_K; ++k) s_e[tid][k] = (valid && k < K) ? __expf(s_e[tid][k] - s_max[4][k]) : 0.f;
+  } else {
 #pragma unroll
-  for (int k = 0; k < MG_K; ++k) s_e[tid][k] = (valid && k < K) ? __expf(lg[k] - s_max[4][k]) : 0.f;
+    for (int k = 0; k < MG_K; ++k) s_e[tid][k] = (valid && k < K) ? __expf(lg[k] - s_max[4][k]) : 0.f;
+  }
   float* pb = a.partial + (((int64_t)b * gridDim.x + blockIdx.x) * K) * (2 + C);
   __syncthreads();
   if (tid < K) {
@@ -503,6 +514,136 @@ __global__ void mhsa_kernel(const T* qkv, const T* dout, T* out, T* dqkv, int L,
   }
 }
 
+// ------------------------------------------------------------------ MHSA over L <= 216 tokens, dim_head 64
+// The map fusion of the ACDC configuration: 3 x 72 tokens, 4 heads of 64.  The tiled scheme above would need K, V,
+// the probability tile, dO and the dK/dV accumulators (~335 KB) at this size, so here one block per (head, batch)
+// stages Q, K, V (and dO) at a 65-float row stride and runs one warp per row: no L x L tile is stored.
+//   forward / dQ pass   warp per query row i: scores over the keys in registers (lane owns keys lane + 32t),
+//                       softmax by shuffles, out_i / dQ_i with the lane owning channels lane and lane + 32; the
+//                       backward keeps {row max, 1 / row sum, D_i = sum_j P_ij dP_ij} per row in shared memory;
+//   dK / dV pass        warp per key row j: P_ij and dS_ij over the queries recomputed from those row statistics.
+constexpr int MH64_D = 64, MH64_LD = MH64_D + 1, MH64_LMAX = 216, MH64_JT = (MH64_LMAX + 31) / 32, MH64_T = 512;
+
+template <typename T>
+__global__ void __launch_bounds__(MH64_T) mhsa64_kernel(const T* qkv, const T* dout, T* out, T* dqkv, int L, int heads, float scale) {
+  extern __shared__ float sm[];
+  const int inner = heads * MH64_D, h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  const int lane = tid & 31, wid = tid >> 5, nw = MH64_T / 32;
+  float* s_q = sm; float* s_k = s_q + L * MH64_LD; float* s_v = s_k + L * MH64_LD;
+  float* s_do = s_v + L * MH64_LD;                   // backward only: [L][65], then [L][3] row statistics
+  float* s_st = s_do + L * MH64_LD;
+  const bool bwd = dout != nullptr;
+  const T* base = qkv + (int64_t)b * L * 3 * inner + h * MH64_D;
+  for (int o = tid; o < L * MH64_D; o += MH64_T) {
+    const int l = o / MH64_D, d = o % MH64_D;
+    s_q[l * MH64_LD + d] = Elem<T>::ld(base + (int64_t)l * 3 * inner + d);
+    s_k[l * MH64_LD + d] = Elem<T>::ld(base + (int64_t)l * 3 * inner + inner + d);
+    s_v[l * MH64_LD + d] = Elem<T>::ld(base + (int64_t)l * 3 * inner + 2 * inner + d);
+    if (bwd) s_do[l * MH64_LD + d] = Elem<T>::ld(dout + ((int64_t)b * L + l) * inner + h * MH64_D + d);
+  }
+  __syncthreads();
+  T* dbase = bwd ? dqkv + (int64_t)b * L * 3 * inner + h * MH64_D : nullptr;
+  for (int i = wid; i < L; i += nw) {
+    const float* qi = s_q + i * MH64_LD;
+    float p[MH64_JT], m = -INFINITY;
+#pragma unroll
+    for (int t = 0; t < MH64_JT; ++t) {
+      const int j = lane + 32 * t;
+      float acc = -INFINITY;
+      if (j < L) {
+        acc = 0.f;
+        const float* kj = s_k + j * MH64_LD;
+#pragma unroll 16
+        for (int d = 0; d < MH64_D; ++d) acc = fmaf(qi[d], kj[d], acc);
+        acc *= scale;
+      }
+      p[t] = acc; m = fmaxf(m, acc);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    float sum = 0.f;
+#pragma unroll
+    for (int t = 0; t < MH64_JT; ++t) { p[t] = __expf(p[t] - m); sum += p[t]; }
+    const float inv = 1.f / warp_sum(sum);
+#pragma unroll
+    for (int t = 0; t < MH64_JT; ++t) p[t] *= inv;
+    if (!bwd) {
+      float o0 = 0.f, o1 = 0.f;
+#pragma unroll
+      for (int t = 0; t < MH64_JT; ++t)
+        for (int src = 0; src < 32; ++src) {
+          const int j = 32 * t + src;
+          const float pj = __shfl_sync(0xffffffffu, p[t], src);
+          if (j < L) { o0 = fmaf(pj, s_v[j * MH64_LD + lane], o0); o1 = fmaf(pj, s_v[j * MH64_LD + lane + 32], o1); }
+        }
+      T* op = out + ((int64_t)b * L + i) * inner + h * MH64_D;
+      Elem<T>::st(op + lane, o0); Elem<T>::st(op + lane + 32, o1);
+      continue;
+    }
+    // dP_ij = <dO_i, V_j>; D_i = sum_j P_ij dP_ij; dS_ij = P_ij (dP_ij - D_i) * scale; dQ_i = sum_j dS_ij K_j
+    const float* gi = s_do + i * MH64_LD;
+    float dp[MH64_JT], dsum = 0.f;
+#pragma unroll
+    for (int t = 0; t < MH64_JT; ++t) {
+      const int j = lane + 32 * t;
+      float acc = 0.f;
+      if (j < L) {
+        const float* vj = s_v + j * MH64_LD;
+#pragma unroll 16
+        for (int d = 0; d < MH64_D; ++d) acc = fmaf(gi[d], vj[d], acc);
+      }
+      dp[t] = acc; dsum = fmaf(p[t], acc, dsum);
+    }
+    const float Di = warp_sum(dsum);
+    float q0 = 0.f, q1 = 0.f;
+#pragma unroll
+    for (int t = 0; t < MH64_JT; ++t) {
+      const float ds = p[t] * (dp[t] - Di) * scale;
+      for (int src = 0; src < 32; ++src) {
+        const int j = 32 * t + src;
+        const float dsj = __shfl_sync(0xffffffffu, ds, src);
+        if (j < L) { q0 = fmaf(dsj, s_k[j * MH64_LD + lane], q0); q1 = fmaf(dsj, s_k[j * MH64_LD + lane + 32], q1); }
+      }
+    }
+    T* dq = dbase + (int64_t)i * 3 * inner;
+    Elem<T>::st(dq + lane, q0); Elem<T>::st(dq + lane + 32, q1);
+    if (lane == 0) { s_st[3 * i] = m; s_st[3 * i + 1] = inv; s_st[3 * i + 2] = Di; }
+  }
+  if (!bwd) return;
+  __syncthreads();
+  // dV_j = sum_i P_ij dO_i ; dK_j = sum_i dS_ij Q_i
+  for (int j = wid; j < L; j += nw) {
+    const float* kj = s_k + j * MH64_LD;
+    const float* vj = s_v + j * MH64_LD;
+    float k0 = 0.f, k1 = 0.f, v0 = 0.f, v1 = 0.f;
+#pragma unroll 1
+    for (int i0 = 0; i0 < L; i0 += 32) {
+      const int i = i0 + lane;
+      float pij = 0.f, ds = 0.f;
+      if (i < L) {
+        float s = 0.f, dp = 0.f;
+        const float* qi = s_q + i * MH64_LD;
+        const float* gi = s_do + i * MH64_LD;
+#pragma unroll 16
+        for (int d = 0; d < MH64_D; ++d) { s = fmaf(qi[d], kj[d], s); dp = fmaf(gi[d], vj[d], dp); }
+        pij = __expf(s * scale - s_st[3 * i]) * s_st[3 * i + 1];
+        ds = pij * (dp - s_st[3 * i + 2]) * scale;
+      }
+      for (int src = 0; src < 32; ++src) {
+        const float ps = __shfl_sync(0xffffffffu, pij, src), dss = __shfl_sync(0xffffffffu, ds, src);
+        const int r = i0 + src;
+        if (r < L) {
+          v0 = fmaf(ps, s_do[r * MH64_LD + lane], v0); v1 = fmaf(ps, s_do[r * MH64_LD + lane + 32], v1);
+          k0 = fmaf(dss, s_q[r * MH64_LD + lane], k0); k1 = fmaf(dss, s_q[r * MH64_LD + lane + 32], k1);
+        }
+      }
+    }
+    T* dk = dbase + (int64_t)j * 3 * inner + inner;
+    Elem<T>::st(dk + lane, k0); Elem<T>::st(dk + lane + 32, k1);
+    Elem<T>::st(dk + inner + lane, v0); Elem<T>::st(dk + inner + lane + 32, v1);
+  }
+}
+
 inline int grid_for(int64_t items, int threads) {
   int64_t g = (items + threads - 1) / threads;
   const int64_t cap = B200SEG_NUM_SMS * 16;
@@ -540,7 +681,7 @@ extern "C" int b200seg_mapgen_fwd(const void* f, int f_ld, int f_coff, const voi
   a.colstat = colstat; a.partial = workspace; a.B = B; a.N = N; a.K = K; a.C = C;
   const int nblk = (int)((N + MG_T - 1) / MG_T);
   cudaStream_t st = as_stream(stream);
-  const int KC = K <= 32 ? 32 : 64;
+  const int KC = K <= 32 ? 32 : (K <= 64 ? 64 : 80);
   const size_t fsm = sizeof(float) * ((size_t)MG_T * (KC + 1) + MG_T * (MG_CC + 1) + 5 * KC);
 #define B200_MAPGEN_FWD(TT, KK)                                                                                \
   do {                                                                                                         \
@@ -548,8 +689,8 @@ extern "C" int b200seg_mapgen_fwd(const void* f, int f_ld, int f_coff, const voi
     mapgen_fwd_kernel<TT, KK><<<dim3(nblk, B), MG_T, fsm, st>>>(a);                                            \
     mapgen_merge_kernel<TT><<<dim3(K, B), 128, 0, st>>>(a, nblk);                                              \
   } while (0)
-  if (dtype == B200SEG_F16) { if (KC == 32) B200_MAPGEN_FWD(__half, 32); else B200_MAPGEN_FWD(__half, 64); }
-  else { if (KC == 32) B200_MAPGEN_FWD(float, 32); else B200_MAPGEN_FWD(float, 64); }
+  if (dtype == B200SEG_F16) { if (KC == 32) B200_MAPGEN_FWD(__half, 32); else if (KC == 64) B200_MAPGEN_FWD(__half, 64); else B200_MAPGEN_FWD(__half, 80); }
+  else { if (KC == 32) B200_MAPGEN_FWD(float, 32); else if (KC == 64) B200_MAPGEN_FWD(float, 64); else B200_MAPGEN_FWD(float, 80); }
 #undef B200_MAPGEN_FWD
   B200_CHECK_LAUNCH("mapgen_fwd");
   return B200SEG_OK;
@@ -570,14 +711,14 @@ extern "C" int b200seg_mapgen_bwd(const void* f, int f_ld, int f_coff, const voi
   a.B = B; a.N = N; a.K = K; a.C = C;
   const int nblk = (int)((N + MG_T - 1) / MG_T);
   cudaStream_t st = as_stream(stream);
-  const int KC = dw_pad <= 32 ? 32 : 64;
+  const int KC = dw_pad <= 32 ? 32 : (dw_pad <= 64 ? 64 : 80);
 #define B200_MAPGEN_BWD(TT, KK)                                                                                \
   do {                                                                                                         \
     B200_CUDA(cudaFuncSetAttribute(mapgen_bwd_kernel<TT, KK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
     mapgen_bwd_kernel<TT, KK><<<dim3(nblk, B), MG_T, smem, st>>>(a);                                           \
   } while (0)
-  if (dtype == B200SEG_F16) { if (KC == 32) B200_MAPGEN_BWD(__half, 32); else B200_MAPGEN_BWD(__half, 64); }
-  else { if (KC == 32) B200_MAPGEN_BWD(float, 32); else B200_MAPGEN_BWD(float, 64); }
+  if (dtype == B200SEG_F16) { if (KC == 32) B200_MAPGEN_BWD(__half, 32); else if (KC == 64) B200_MAPGEN_BWD(__half, 64); else B200_MAPGEN_BWD(__half, 80); }
+  else { if (KC == 32) B200_MAPGEN_BWD(float, 32); else if (KC == 64) B200_MAPGEN_BWD(float, 64); else B200_MAPGEN_BWD(float, 80); }
 #undef B200_MAPGEN_BWD
   B200_CHECK_LAUNCH("mapgen_bwd");
   return B200SEG_OK;
@@ -685,6 +826,19 @@ extern "C" int b200seg_mhsa(const void* qkv, const void* dout, void* out, void* 
                             float scale, int dtype, void* stream) {
   if (!qkv || B <= 0 || L <= 0 || heads <= 0 || !ok_dtype(dtype)) return B200SEG_EINVAL;
   if ((dout == nullptr) == (out == nullptr) || (dout && !dqkv)) return B200SEG_EINVAL;
+  if (dim_head == MH64_D) {
+    if (L > MH64_LMAX || heads > 65535 || B > 65535) return B200SEG_EUNSUPPORTED;
+    const size_t smem = sizeof(float) * ((size_t)(dout ? 4 : 3) * L * MH64_LD + (dout ? 3 * (size_t)L : 0));
+    if (dtype == B200SEG_F16) {
+      B200_CUDA(cudaFuncSetAttribute(mhsa64_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      mhsa64_kernel<__half><<<dim3(heads, B), MH64_T, smem, as_stream(stream)>>>((const __half*)qkv, (const __half*)dout, (__half*)out, (__half*)dqkv, L, heads, scale);
+    } else {
+      B200_CUDA(cudaFuncSetAttribute(mhsa64_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      mhsa64_kernel<float><<<dim3(heads, B), MH64_T, smem, as_stream(stream)>>>((const float*)qkv, (const float*)dout, (float*)out, (float*)dqkv, L, heads, scale);
+    }
+    B200_CHECK_LAUNCH("mhsa");
+    return B200SEG_OK;
+  }
   if (dim_head != MH_D || L > 192) return B200SEG_EUNSUPPORTED;
   const size_t smem = sizeof(float) * ((size_t)(dout ? 6 : 3) * L * (MH_D + 1) + (size_t)MH_RT * (L + 1));
   if (dtype == B200SEG_F16) {

@@ -4,8 +4,10 @@ Same constructor arguments, the same module tree / parameter registration order,
 `state_dict()` keys and shapes as the reference, so checkpoints, EMA zipping and DDP buckets are interchangeable
 (SURVEY.md §8b).  The forward is written against libb200seg only: dense convs on the tensor-core path, depthwise convs,
 B-MHA, map generation, SE, the token transformer — each a torch.autograd.Function from medformer_ops.py / ops.py.
-Supported configuration = what every reference MedFormer YAML uses: norm 'in', act 'relu', conv_block
-'BasicBlock', proj_type 'depthwise', dropout 0, dim_head 32 on attention levels, <= 64 map tokens.
+Supported configuration = what the reference MedFormer YAMLs for BCV, AMOS, KiTS and ACDC use: norm 'in', act 'relu',
+conv_block 'BasicBlock', proj_type 'depthwise', dropout 0, dim_head 32, 64 or 80 on attention levels, <= 80 map tokens,
+and a map-fusion attention of dim_head 32 over <= 192 fused tokens or dim_head 64 over <= 216.  LiTS (one head of
+128..320 channels) raises ValueError.
 """
 import torch
 import torch.nn as nn
@@ -19,6 +21,16 @@ from .unet3d import BasicBlock, ConvNormAct, _check_kernel, _triple
 
 EPS_BLOCK = 1e-4      # ConvNormAct's norm(in_ch, eps=1e-4), conv_layers.py:40
 EPS_PLAIN = 1e-5      # bare norm(dim): PatchMerging.norm :158, BidirectionAttentionBlock.norm1/2 :107-108
+BIATTN_DIM_HEADS = (32, 64, 80)     # csrc/biattn.cu: the original kernels (32, <= 64 tokens) and the wide ones
+BIATTN_MAX_TOKENS = 80              # map tokens of B-MHA and map generation
+MHSA_MAX_TOKENS = {32: 192, 64: 216}    # fused map tokens of the map-fusion attention per dim_head (b200seg_mhsa)
+
+
+def _prod(size):
+    n = 1
+    for s in size:
+        n *= int(s)
+    return n
 
 
 def _conv(pack, x, stats, weights, ksize, act=ACT_NONE, bias=None, residual=None, co_pad=0, eps=EPS_BLOCK,
@@ -61,8 +73,10 @@ class BidirectionAttention(nn.Module):
         super().__init__()
         if proj_type != 'depthwise':
             raise ValueError("the H100 path implements proj_type='depthwise' only")
-        if dim_head != 32:
-            raise ValueError("the B-MHA kernel needs dim_head == 32 (got %d)" % dim_head)
+        if dim_head not in BIATTN_DIM_HEADS:
+            raise ValueError("the B-MHA kernels need dim_head in %s (got %d)" % (BIATTN_DIM_HEADS, dim_head))
+        if _prod(map_size) > BIATTN_MAX_TOKENS:
+            raise ValueError("the B-MHA kernels handle at most %d map tokens, got map_size=%s" % (BIATTN_MAX_TOKENS, map_size))
         self.inner_dim = dim_head * heads
         self.heads, self.dim_head = heads, dim_head
         self.feat_qv = DepthwiseSeparableConv(feat_dim, self.inner_dim * 2, kernel_size=kernel_size)
@@ -201,8 +215,8 @@ class SemanticMapGeneration(nn.Module):
         self.map_size = tuple(map_size)
         self.map_dim = map_dim
         self.map_code_num = map_size[0] * map_size[1] * map_size[2]
-        if self.map_code_num > 64:
-            raise ValueError("the map kernels handle at most 64 map tokens, got map_size=%s" % (map_size,))
+        if self.map_code_num > BIATTN_MAX_TOKENS:
+            raise ValueError("the map kernels handle at most %d map tokens, got map_size=%s" % (BIATTN_MAX_TOKENS, map_size))
         self.base_proj = nn.Conv3d(feat_dim, map_dim, kernel_size=3, padding=1, bias=False)
         self.semantic_proj = nn.Conv3d(feat_dim, self.map_code_num, kernel_size=3, padding=1, bias=False)
         self._pack = PackedWeights()
@@ -228,8 +242,8 @@ class Attention(nn.Module):
 
     def __init__(self, dim, heads, dim_head):
         super().__init__()
-        if dim_head != 32:
-            raise ValueError("the token attention kernel needs dim_head == 32")
+        if dim_head not in MHSA_MAX_TOKENS:
+            raise ValueError("the token attention kernels need dim_head in %s (got %d)" % (tuple(MHSA_MAX_TOKENS), dim_head))
         self.heads, self.dim_head = heads, dim_head
         inner = dim_head * heads
         self.to_qkv = _Linear(dim, inner * 3, bias=False)
@@ -345,8 +359,8 @@ class down_block(nn.Module):
             self.map_gen = SemanticMapGeneration(out_ch, map_dim, map_size)
         self.patch_merging = PatchMerging(in_ch, out_ch, proj_type=proj_type, down_scale=down_scale, kernel_size=kernel_size)
         self.conv_blocks = nn.Sequential(*[BasicBlock(out_ch, out_ch, kernel_size=kernel_size) for _ in range(conv_num)])
-        if trans_num and dim_head != 32:
-            raise ValueError("attention levels need dim_head == 32")
+        if trans_num and dim_head not in BIATTN_DIM_HEADS:
+            raise ValueError("attention levels need dim_head in %s (got %d)" % (BIATTN_DIM_HEADS, dim_head))
         self.trans_blocks = BasicLayer(out_ch, map_dim, out_ch, num_blocks=trans_num, heads=heads,
                                        dim_head=dim_head if trans_num else 32, expansion=expansion, map_size=map_size,
                                        proj_type=proj_type, kernel_size=kernel_size)
@@ -421,6 +435,10 @@ class MedFormer(nn.Module):
                                 heads=num_heads[2], dim_head=dim_head[2], map_generate=True, **common)
         self.down4 = down_block(chan_num[2], chan_num[3], conv_num[3], trans_num[3], kernel_size=ks[4], down_scale=sc[3],
                                 heads=num_heads[3], dim_head=dim_head[3], map_generate=True, **common)
+        fused, fdh = 3 * _prod(map_size), fusion_dim // fusion_heads
+        if fdh in MHSA_MAX_TOKENS and fused > MHSA_MAX_TOKENS[fdh]:
+            raise ValueError("the map-fusion attention at dim_head %d handles at most %d tokens, got 3 x %d"
+                             % (fdh, MHSA_MAX_TOKENS[fdh], _prod(map_size)))
         self.map_fusion = SemanticMapFusion(chan_num[1:4], fusion_dim, fusion_heads, depth=fusion_depth)
         self.up1 = up_block(chan_num[3], chan_num[4], conv_num[4], trans_num[4], kernel_size=ks[3], up_scale=sc[3],
                             heads=num_heads[4], dim_head=dim_head[4], map_shortcut=True, **common)

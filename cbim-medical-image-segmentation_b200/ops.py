@@ -655,6 +655,49 @@ def biattn_bwd(fqv, mqv, mo, colstat, dfo, dmo, heads, dim_head=32):
     return dfqv, dmqv
 
 
+def biattn_wide_fwd(fqv, mqv, heads, dim_head):
+    """biattn_fwd for the shapes b200seg_biattn_fwd refuses (dim_head 64 / 80, or more than 64 map tokens at 32)."""
+    _need_cuda(fqv)
+    inner = heads * dim_head
+    B = fqv.shape[0]
+    N = fqv.numel() // (B * fqv.shape[-1])
+    M = mqv.numel() // (B * mqv.shape[-1])
+    assert fqv.shape[-1] == 2 * inner and mqv.shape[-1] == 2 * inner and fqv.dtype == mqv.dtype
+    fo = torch.empty(*fqv.shape[:-1], inner, dtype=fqv.dtype, device=fqv.device)
+    mo = torch.empty(*mqv.shape[:-1], inner, dtype=fqv.dtype, device=fqv.device)
+    colstat = torch.empty(B, heads, M, 2, dtype=torch.float32, device=fqv.device)
+    ws = torch.empty(_lib.load().b200seg_biattn_wide_workspace(B, N, M, heads, dim_head), dtype=torch.uint8,
+                     device=fqv.device)
+    call("b200seg_biattn_wide_fwd", fqv.data_ptr(), 2 * inner, 0, fqv.data_ptr(), 2 * inner, inner,
+         mqv.data_ptr(), 0, mqv.data_ptr(), inner, 2 * inner, fo.data_ptr(), inner, 0, mo.data_ptr(), inner, 0,
+         colstat.data_ptr(), ws.data_ptr(), B, N, M, heads, dim_head, float(dim_head) ** -0.5, _dt(fqv), _stream())
+    return fo, mo, colstat
+
+
+def biattn_wide_bwd(fqv, mqv, mo, colstat, dfo, dmo, heads, dim_head):
+    inner = heads * dim_head
+    B = fqv.shape[0]
+    N = fqv.numel() // (B * fqv.shape[-1])
+    M = mqv.numel() // (B * mqv.shape[-1])
+    dfqv = torch.empty_like(fqv)
+    dmqv = torch.empty_like(mqv)
+    ws = torch.empty(_lib.load().b200seg_biattn_wide_workspace(B, N, M, heads, dim_head), dtype=torch.uint8,
+                     device=fqv.device)
+    call("b200seg_biattn_wide_bwd", fqv.data_ptr(), 2 * inner, 0, fqv.data_ptr(), 2 * inner, inner,
+         mqv.data_ptr(), 0, mqv.data_ptr(), inner, 2 * inner, mo.data_ptr(), inner, 0, colstat.data_ptr(),
+         dfo.data_ptr(), inner, 0, dmo.data_ptr(), inner, 0,
+         dfqv.data_ptr(), 2 * inner, 0, dfqv.data_ptr(), 2 * inner, inner,
+         dmqv.data_ptr(), 0, dmqv.data_ptr(), inner, 2 * inner,
+         ws.data_ptr(), B, N, M, heads, dim_head, float(dim_head) ** -0.5, _dt(fqv), _stream())
+    return dfqv, dmqv
+
+
+def biattn_is_wide(dim_head, M):
+    """Which B-MHA entry owns a shape: the original one-voxel-per-thread kernels keep dim_head 32 with <= 64 map tokens
+    (every BCV / AMOS / KiTS level, bit for bit as before); everything else goes to the wide kernels."""
+    return not (dim_head == 32 and M <= 64)
+
+
 class BiAttnFn(torch.autograd.Function):
     """Differentiable B-MHA core on channels-last tensors (medformer_utils.py:63-97 minus the projections)."""
 
@@ -662,15 +705,18 @@ class BiAttnFn(torch.autograd.Function):
     def forward(ctx, fqv, mqv, heads, dim_head):
         fqv = fqv.contiguous()
         mqv = mqv.contiguous()
-        fo, mo, colstat = biattn_fwd(fqv, mqv, heads, dim_head)
+        wide = biattn_is_wide(dim_head, mqv.numel() // (mqv.shape[0] * mqv.shape[-1]))
+        fo, mo, colstat = (biattn_wide_fwd if wide else biattn_fwd)(fqv, mqv, heads, dim_head)
         ctx.save_for_backward(fqv, mqv, mo, colstat)
         ctx.hd = (heads, dim_head)
+        ctx.wide = wide
         return fo, mo
 
     @staticmethod
     def backward(ctx, dfo, dmo):
         fqv, mqv, mo, colstat = ctx.saved_tensors
-        dfqv, dmqv = biattn_bwd(fqv, mqv, mo, colstat, dfo.contiguous(), dmo.contiguous(), *ctx.hd)
+        bwd = biattn_wide_bwd if ctx.wide else biattn_bwd
+        dfqv, dmqv = bwd(fqv, mqv, mo, colstat, dfo.contiguous(), dmo.contiguous(), *ctx.hd)
         return dfqv, dmqv, None, None
 
 

@@ -345,6 +345,27 @@ int b200seg_biattn_bwd(const void* fq, int fq_ld, int fq_coff, const void* fv, i
                        float* workspace, int B, int64_t N, int M, int heads, int dim_head, float scale,
                        int dtype, void* stream);
 
+/* Wide B-MHA: the same operands and conventions as b200seg_biattn_fwd / _bwd for the
+ * shapes those refuse: dim_head 32 with 65..80 map tokens, dim_head 64 or 80 with
+ * 1..80 map tokens (ACDC's 2x6x6 maps at dim_head 32 / 64 / 80).  Every other shape,
+ * dim_head 32 with M <= 64 included, returns B200SEG_EUNSUPPORTED, so each shape has
+ * exactly one path.  workspace: b200seg_biattn_wide_workspace() bytes; it takes
+ * dim_head because the per-block partials are 2*dim_head floats per map token. */
+size_t b200seg_biattn_wide_workspace(int B, int64_t N, int M, int heads, int dim_head);
+int b200seg_biattn_wide_fwd(const void* fq, int fq_ld, int fq_coff, const void* fv, int fv_ld, int fv_coff,
+                            const void* mq, int mq_coff, const void* mv, int mv_coff, int m_ld,
+                            void* fo, int fo_ld, int fo_coff, void* mo, int mo_ld, int mo_coff,
+                            float* colstat, float* workspace, int B, int64_t N, int M, int heads, int dim_head,
+                            float scale, int dtype, void* stream);
+int b200seg_biattn_wide_bwd(const void* fq, int fq_ld, int fq_coff, const void* fv, int fv_ld, int fv_coff,
+                            const void* mq, int mq_coff, const void* mv, int mv_coff, int m_ld,
+                            const void* mo, int mo_ld, int mo_coff, const float* colstat,
+                            const void* dfo, int dfo_ld, int dfo_coff, const void* dmo, int dmo_ld, int dmo_coff,
+                            void* dfq, int dfq_ld, int dfq_coff, void* dfv, int dfv_ld, int dfv_coff,
+                            void* dmq, int dmq_coff, void* dmv, int dmv_coff, int dm_ld,
+                            float* workspace, int B, int64_t N, int M, int heads, int dim_head, float scale,
+                            int dtype, void* stream);
+
 /* ---------------------------------------------------------------------------
  * Depthwise 3-D convolution (groups == C), stride 1, "same" padding, no bias:
  * DepthwiseSeparableConv.depthwise conv_layers.py:135-143 (MedFormer attention
@@ -371,7 +392,7 @@ int b200seg_dwconv3d_wgrad(const void* x, int x_ld, int x_coff, const double* x_
  *   y[b,d,h,w,q*C+c] = x[b,d*sd+i,h*sh+j,w*sw+k,c], q=(i*sh+j)*sw+k; reverse!=0
  *   scatters y back into x (the gradient).  Do/Ho/Wo are the OUTPUT extents.
  * mapgen: SemanticMapGeneration medformer_utils.py:221-226,
- *   map[b,k,c] = sum_j softmax_j(wl[b,j,k]) * f[b,j,c]   (K <= 64 map codes),
+ *   map[b,k,c] = sum_j softmax_j(wl[b,j,k]) * f[b,j,c]   (K <= 80 map codes),
  *   colstat float[B][K][2]; bwd writes df and dwl (dw_pad >= K logits channels,
  *   the padding gets zeros) into the gradient of the fused projection output.
  * se_gate: SEBlock conv_layers.py:159-174 on the channel means taken from IN
@@ -383,7 +404,8 @@ int b200seg_dwconv3d_wgrad(const void* x, int x_ld, int x_coff, const double* x_
  * layernorm: nn.LayerNorm(C, eps) trans_layers.py:36-41 over rows [R][C];
  *   mean_rstd float[R][2]; bwd accumulates (+=) dgamma/dbeta.
  * gelu: exact erf GELU trans_layers.py:22; dy==NULL -> forward, else out=dy*gelu'(x).
- * mhsa: Attention core trans_layers.py:84-93 for L<=192 tokens, dim_head 32;
+ * mhsa: Attention core trans_layers.py:84-93 for dim_head 32 with L<=192 tokens
+ *   and dim_head 64 with L<=216 tokens;
  *   qkv [B][L][3*inner] ('(heads dim_head)' order), out [B][L][inner];
  *   forward when dout==NULL, otherwise writes dqkv.
  * ------------------------------------------------------------------------- */
